@@ -4,11 +4,17 @@
 // differs between instances (G1: 91 % need one iteration, 1 in 10 000 needs six or more), and with a static round-robin
 // the warp that meets a slow instance also keeps its whole share of ordinary tiles, which set the kernel time.  The last
 // CTA to leave (sched[1] counts them) rewinds the counter for the next launch on the stream.
+//
+// The kernel is bound by instruction issue and fetch, so its code size is part of its speed.  bik_step, bik_step_host and
+// bik_converge launch a STEP instantiation (fp64 solve, fp32 buffers, packed rows, default solver settings) that leaves out
+// the code of the other forms, keeps one-off work out of line and does not unroll the solver loops: 9 216 SASS instructions
+// on sm_90a for G = 8 instead of 17 592, and K2 in the G1 step 0.60 ms instead of 0.78 ms on one H100 80GB HBM3 (SXM, 700 W
+// power limit).  tests/test_k2_code_size_cpu.py keeps it that size.
 #include "bik_dev.cuh"
 
 using namespace bik;
 
-template <typename T, int G, int MAXT, typename M, bool F32IO>
+template <typename T, int G, int MAXT, typename M, bool F32IO, bool STEP>
 __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_kernel(const uint32_t* __restrict__ gimage, int warp_bytes, K2Args a, unsigned int* sched) {
   extern __shared__ __align__(16) uint32_t smem[];
   constexpr int NS = 32 / G;
@@ -24,17 +30,17 @@ __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_kernel(const uint32_t* _
       if (lane == 0) t = atomicAdd(&sched[0], 1u);
       t = __shfl_sync(0xffffffffu, t, 0);
       if ((long long)t >= ntiles) break;
-      k2t_warp_tile<T, G, NS, M, F32IO>(P, a, (long long)t * NS, wsm, lane, St, uw);
+      k2t_warp_tile<T, G, NS, M, F32IO, STEP>(P, a, (long long)t * NS, wsm, lane, St, uw);
     }
     __syncthreads();
     if (threadIdx.x == 0 && atomicInc(&sched[1], gridDim.x - 1) == gridDim.x - 1) { __threadfence(); sched[0] = 0u; }
     return;
   }
   for (long long tile = (long long)blockIdx.x * nwarps + warp; tile < ntiles; tile += (long long)gridDim.x * nwarps)
-    k2t_warp_tile<T, G, NS, M, F32IO>(P, a, tile * NS, wsm, lane, St, uw);
+    k2t_warp_tile<T, G, NS, M, F32IO, STEP>(P, a, tile * NS, wsm, lane, St, uw);
 }
 
-template <typename T, int G, typename M, bool F32IO>
+template <typename T, int G, typename M, bool F32IO, bool STEP>
 static int launch_k2t_io(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
   constexpr int NS = 32 / G, MAXT = sizeof(T) == 8 ? 256 : 512;
   PView P{p->image.data()};
@@ -44,16 +50,21 @@ static int launch_k2t_io(const bik_problem* p, const K2Args& a, unsigned int* sc
   const size_t smem = NW * wb;
   int grid = 1;
   long long tiles = ((long long)a.B + NS - 1) / NS;
-  int rc = bik_launch_geometry((const void*)k2t_kernel<T, G, MAXT, M, F32IO>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
+  int rc = bik_launch_geometry((const void*)k2t_kernel<T, G, MAXT, M, F32IO, STEP>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
   if (rc) return rc;
-  k2t_kernel<T, G, MAXT, M, F32IO><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
+  k2t_kernel<T, G, MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
 template <typename T, int G, typename M>
 static int launch_k2t(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
-  if (sizeof(T) == 4 || !(a.io64 || a.pk64 || a.dense64)) return launch_k2t_io<T, G, M, true>(p, a, sched, st);   // fp32 buffers everywhere
-  return launch_k2t_io<T, G, M, sizeof(T) == 4>(p, a, sched, st);
+  if (sizeof(T) == 4 || !(a.io64 || a.pk64 || a.dense64)) {   // fp32 buffers everywhere
+    // the step's form (packed rows from K1, active-set guess, primal pivoting rule): the fp64 solve without the other forms' code
+    const bool step = sizeof(T) == 8 && a.pk && !a.ep && p->h.k2_sweeps > 0 && p->h.k2_rule == 1;
+    if (step) return launch_k2t_io<T, G, M, true, sizeof(T) == 8>(p, a, sched, st);
+    return launch_k2t_io<T, G, M, true, false>(p, a, sched, st);
+  }
+  return launch_k2t_io<T, G, M, sizeof(T) == 4, false>(p, a, sched, st);
 }
 static int group_of(const bik_problem* p) { return (p->h.nu > K2T_NMAX || p->k2_group == 8) ? 8 : 4; }
 static bool use_double(const bik_problem* p, const K2Args& a) { return p->solve_double || a.io64 || a.pk64 || a.dense64 || p->h.nu > K2T_NMAX; }

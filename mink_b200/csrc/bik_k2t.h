@@ -38,12 +38,6 @@
 #define BIK_WARP_ANY(x) (x)
 #endif
 
-#ifdef BIK_K2T_UNROLL1
-#define BIK_K2T_LOOP _Pragma("unroll 1")
-#else
-#define BIK_K2T_LOOP
-#endif
-
 namespace bik {
 
 BIK_HD uint32_t bik_float_bits(float f) {
@@ -112,6 +106,7 @@ template <typename T, int G> BIK_HD T grp_sum(T v) {
 BIK_HD int k2t_task_tile_words(const PView& P) {  // widest task tile, in T words per instance (odd)
   const PHeader& h = P.h();
   int m = 1;
+  #pragma unroll 1
   for (int f = 0; f < h.F; ++f) { int ne = 6 * P.frame(f).ncols + 6; m = ne > m ? ne : m; }
   if (h.C > 0) { int ne = 3 * h.com_ncols + 3; m = ne > m ? ne : m; }
   return m | 1;
@@ -133,8 +128,8 @@ BIK_HD int k2t_warp_bytes(const PView& P, int ts, int NS) { return (NS * k2t_slo
 // One task's weighted block, column-major like K1's packed record:
 //   tile[i][ia*nr + r] = cost_r J[row0+r][col_ia],   tile[i][nr*nc + r] = cost_r (-gain e[row0+r]).
 // Source: the packed hand-off (one contiguous run per instance: coalesced without any index arithmetic) or, for bik_solve,
-// the dense rows (gather through the task's column list).
-template <typename T, int W, int NS>
+// the dense rows (gather through the task's column list).  PK: the packed hand-off is known to be there.
+template <typename T, int W, int NS, bool PK = false>
 BIK_HD void k2t_stage_task(T* tile, int S, int lane, int cnt, long long b0, const K2Args& a, int pk64, int dense64, int K, int nv, int pks,
                            const int32_t* cols, const K2Task& tk) {
   const int nj = tk.nr * tk.nc, ne = nj + tk.nr;
@@ -142,7 +137,7 @@ BIK_HD void k2t_stage_task(T* tile, int S, int lane, int cnt, long long b0, cons
     const int ia = k / tk.nr, r = k - ia * tk.nr;
     const bool isj = k < nj;
     const T cr = isj ? T(tk.cost[r]) : T(tk.cost[r]) * T(-tk.gain);
-    if (a.pk) {
+    if (PK || a.pk) {
       const long long o = b0 * pks + tk.pk_off + k;
 #pragma unroll
       for (int i = 0; i < NS; ++i) tile[i * S + k] = i < cnt ? cr * ldin<T>(a.pk, o + (long long)i * pks, pk64) : T(0);
@@ -186,7 +181,7 @@ BIK_HD void k2t_task_accumulate_nr(const T* tr, int nc, const int32_t* cols, con
     for (int r = 0; r < NR; ++r) { col[r] = tr[ia * NR + r]; cs += wev[r] * col[r]; }
     const int ua = umap[cols[ia] & 0xffff];
     c[ua * NS] -= cs;
-    BIK_K2T_LOOP
+    #pragma unroll 1
     for (int ib = 0; ib <= ia; ++ib) {
       const T* cb = tr + ib * NR;
       T s = T(0);
@@ -198,16 +193,25 @@ BIK_HD void k2t_task_accumulate_nr(const T* tr, int nc, const int32_t* cols, con
     }
   }
 }
+// The CoM task (at most one per problem) is assembled out of line: its unrolled copy would otherwise sit in the kernel
+// beside the frame tasks' one.
+template <typename T, int G, int NS>
+BIK_NOINLINE void k2t_task_accumulate_com(const T* tr, int nc, const int32_t* cols, const int32_t* umap, T* Hp, T* c, int l) {
+  BIK_IN_SHARED(tr); BIK_IN_SHARED(Hp); BIK_IN_SHARED(c);
+  k2t_task_accumulate_nr<T, G, NS, 3>(tr, nc, cols, umap, Hp, c, l);
+}
 template <typename T, int G, int NS>
 BIK_HD void k2t_task_accumulate(const T* tr, int nr, int nc, const int32_t* cols, const int32_t* umap, T* Hp, T* c, float lm, T* mu, int l) {
   const T* wev = tr + nr * nc;
   if (lm != 0.f) { T s = T(0); for (int r = 0; r < nr; ++r) s += wev[r] * wev[r]; *mu += T(lm) * s; }
   if (nr == 6) k2t_task_accumulate_nr<T, G, NS, 6>(tr, nc, cols, umap, Hp, c, l);
-  else k2t_task_accumulate_nr<T, G, NS, 3>(tr, nc, cols, umap, Hp, c, l);   // CoM task
+  else k2t_task_accumulate_com<T, G, NS>(tr, nc, cols, umap, Hp, c, l);
 }
 
 // ---- solver pieces: compact run-time loops (the whole pivoting iteration must stay resident in the
-// instruction cache -- the fully unrolled variants of these routines were instruction-fetch bound) --------
+// instruction cache -- the fully unrolled variants of these routines were instruction-fetch bound).  Every loop here and in
+// the assembly carries `#pragma unroll 1`: unrolled by the compiler they made the step's kernel 17.6 k SASS instructions on
+// sm_90a, and even the factor's and the assembly's dot loops alone cost 6 % of K2's time in the G1 step on an H100 --------
 // Dot product of row i of the symmetric packed matrix with a vector (both slot-strided in shared memory).
 #ifdef BIK_K2T_NOINLINE_ROWDOT
 #define BIK_K2T_ROWDOT_ATTR BIK_NOINLINE
@@ -225,11 +229,11 @@ BIK_K2T_ROWDOT_ATTR T k2t_row_dot(const T* __restrict__ Hp, const T* __restrict_
   const T* pv = v + k0 * NS;
   T a0 = T(0), a1 = T(0);
   int k = i + 1 - k0;
-  BIK_K2T_LOOP
+  #pragma unroll 1
   for (; k >= 2; k -= 2) { a0 += row[0] * pv[0]; a1 += row[NS] * pv[NS]; row += 2 * NS; pv += 2 * NS; }
   if (k) { a0 += row[0] * pv[0]; pv += NS; }
   const T* col = Hp + (tri(i + 1) + i) * NS;   // entries (m, i), m > i, sit at tri(m) + i
-  BIK_K2T_LOOP
+  #pragma unroll 1
   for (int m = i + 1; m < nu; ++m) { a1 += col[0] * pv[0]; col += (m + 1) * NS; pv += NS; }
   return a0 + a1;
 }
@@ -267,7 +271,7 @@ BIK_K2T_FACTOR_ATTR int k2t_factor(const T* __restrict__ Hp, T* __restrict__ Lp,
         const T* pi = dst + kb * NS;
         T a0 = T(0), a1 = T(0);
         int m = k - kb;
-        BIK_K2T_LOOP
+        #pragma unroll 1
         for (; m >= 2; m -= 2) { a0 += pi[0] * pk[0]; a1 += pi[NS] * pk[NS]; pi += 2 * NS; pk += 2 * NS; }
         if (m) { a0 += pi[0] * pk[0]; pk += NS; }
         s = (src[k * NS] - (a0 + a1)) * pk[0];   // pk now points at 1 / L[k][k]
@@ -303,7 +307,7 @@ BIK_HD void k2t_backsub(T* __restrict__ Lp, int nu, int l, T* __restrict__ xs, i
   for (int k = khi - 1; k >= klo; --k) {
     const T* row = Lp + tri(k) * NS;
     const T xk = y[k * NS] * row[k * NS];
-    BIK_K2T_LOOP
+    #pragma unroll 1
     for (int m = mlo + l; m < k; m += G) y[m * NS] -= row[m * NS] * xk;
     if (l == 0) xs[k * NS] = xk;
     if (G > 1) BIK_SYNCWARP();   // y_{k-1} is final
@@ -316,6 +320,7 @@ BIK_HD void k2t_backsub_cross(T* __restrict__ Lp, int nu, int l, const T* __rest
   T* y = Lp + tri(nu) * NS;
   for (int m = l; m < mhi; m += G) {
     T a = y[m * NS];
+    #pragma unroll 1
     for (int k = klo; k < khi; ++k) a -= Lp[(tri(k) + m) * NS] * xs[k * NS];
     y[m * NS] = a;
   }
@@ -354,7 +359,7 @@ BIK_HD void k2t_pgs_guess(const T* __restrict__ Hp, const T* __restrict__ c, con
       else if (xi >= bu) { xi = bu; upm |= M(1) << i; }
       const T dx = xi - xo;
       if (G > 1) BIK_SYNCWARP();   // every lane has read res_i and x_i
-      BIK_K2T_LOOP
+      #pragma unroll 1
       for (int m = k0 + l; m < nu; m += G) {
         const int hi_ = m > i ? m : i, lo_ = m > i ? i : m;
         res[m * NS] += Hp[(tri(hi_) + lo_) * NS] * dx;
@@ -379,7 +384,7 @@ BIK_HD void k2t_schur(T* __restrict__ Hp, const T* __restrict__ Lp, T* __restric
     for (int j = nf + l; j <= i + 1; j += G) {       // j == i + 1 stands for the linear term
       const T* pj = j <= i ? Lp + tri(j) * NS : y;
       T a0 = T(0);
-      BIK_K2T_LOOP
+      #pragma unroll 1
       for (int m = 0; m < nf; ++m) a0 += pi[m * NS] * pj[m * NS];
       if (j <= i) Hp[(tri(i) + j) * NS] -= a0;
       else c[i * NS] += a0;
@@ -387,12 +392,46 @@ BIK_HD void k2t_schur(T* __restrict__ Hp, const T* __restrict__ Lp, T* __restric
   }
 }
 
+// ---- work that runs once per tile, or for few problems: out of line, so that it does not take instruction-cache room
+// from the solver loops.  Same arithmetic as in line.
+// Levenberg-Marquardt terms of the posture tasks: mu + sum_p lm_p |W_p e_p|^2 (eprow: the staged posture errors).
+template <typename T>
+BIK_NOINLINE T k2t_posture_lm(PView P, const T* eprow, T mu) {
+  BIK_IN_SHARED(eprow);
+  const PHeader& h = P.h();
+  const int nv = h.nv;
+  #pragma unroll 1
+  for (int p = 0; p < h.P; ++p) {
+    const float* pr = P.f(h.off_posture) + p * (2 + nv);
+    if (pr[1] != 0.f) {
+      T s = T(0);
+      #pragma unroll 1
+      for (int d = 0; d < nv; ++d) { T v = T(pr[2 + d]) * T(pr[0]) * eprow[p * nv + d]; s += v * v; }
+      mu += T(pr[1]) * s;
+    }
+  }
+  return mu;
+}
+// q <- q (+) dq of one free or ball joint (quaternion update)
+template <typename T>
+BIK_NOINLINE void k2t_integrate_quat_node(const NodeRec& r, T* q, const T* dq) { integrate_node(r, q, dq); }
+// Active set left for the next step's warm start: 0 free, 1 lower, 2 upper, +4 = a.dq holds this step's result
+template <typename M>
+BIK_NOINLINE void k2t_store_warm(signed char* wm, int nu, M lom, M upm) {
+  #pragma unroll 1
+  for (int i = 0; i < nu; ++i) wm[i] = (signed char)((((lom >> i) & M(1)) ? 1 : (((upm >> i) & M(1)) ? 2 : 0)) | 4);
+}
+
 // ---- one tile of NS instances per warp ----------------------------------------------------------------
 // F32IO (compile time): every caller buffer and the hand-off hold fp32 -- the batched fast path: the fp64 load / store /
 // integrate code is not even compiled in (it tripled the kernel's SASS and its instruction-fetch stalls).  Otherwise the
 // element types follow the run-time flags of K2Args.
-template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false>
+// STEP (compile time, with F32IO and T = double): the form bik_step / bik_step_host / bik_converge launch with the default
+// solver settings -- packed task rows (a.pk set, a.ep null), k2_sweeps > 0, k2_rule == 1.  Only the packed staging and the
+// guessed primal active-set loop are compiled in: no dense-row staging, no block-flip branch, no warm-mask decode.
+template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false>
 BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* wsm, int lane, int St = 0, int uw = 0) {
+  static_assert(!STEP || (F32IO && sizeof(T) == 8), "the step instantiation is fp64 on fp32 buffers");
   if (St == 0) { St = k2t_task_tile_words(P); uw = k2t_union_words(P, sizeof(T)); }   // callers that loop over tiles pass them in
   const int io64 = F32IO ? 0 : a.io64, pk64 = F32IO ? 0 : a.pk64, dense64 = F32IO ? 0 : a.dense64;
   constexpr int W = G * NS;
@@ -418,13 +457,15 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   float* const hi = Fb + (size_t)nu * NS + slot;
 
   // ---- assembly ----
+  #pragma unroll 1
   for (int k = l; k < tri(nu); k += G) Hp[k * NS] = T(0);
+  #pragma unroll 1
   for (int k = l; k < nu; k += G) c[k * NS] = T(0);
   T mu = T(a.damping);
   for (int t = 0; t < h.F + h.C; ++t) {
     const K2Task tk = k2_task(P, t);
     BIK_SYNCWARP();
-    k2t_stage_task<T, W, NS>(U, St, lane, cnt, b0, a, pk64, dense64, K, nv, h.pk_stride, cols + tk.coff, tk);
+    k2t_stage_task<T, W, NS, STEP>(U, St, lane, cnt, b0, a, pk64, dense64, K, nv, h.pk_stride, cols + tk.coff, tk);
     BIK_SYNCWARP();
     k2t_task_accumulate<T, G, NS>(U + (size_t)slot * St, tk.nr, tk.nc, cols + tk.coff, umap, Hp, c, tk.lm, &mu, l);
   }
@@ -432,9 +473,9 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   BIK_SYNCWARP();
   const int Sq = (nq + NP * nv) | 1;
   k2t_stage_q<T, W, NS>(U, Sq, lane, cnt, a.q, io64, b0, nq);
-  if (NP > 0 && a.ep) k2t_stage_rows<T, W, NS>(U, Sq, nq, lane, cnt, a.ep, dense64, b0 * NP * nv, (long long)NP * nv, NP * nv);
+  if (!STEP && NP > 0 && a.ep) k2t_stage_rows<T, W, NS>(U, Sq, nq, lane, cnt, a.ep, dense64, b0 * NP * nv, (long long)NP * nv, NP * nv);
   BIK_SYNCWARP();
-  if (NP > 0 && !a.ep) {   // inside bik_step K1 hands no posture error over: e = q* (-) q from the staged q (posture_task.py:107-118)
+  if (NP > 0 && (STEP || !a.ep)) {   // inside bik_step K1 hands no posture error over: e = q* (-) q from the staged q (posture_task.py:107-118)
     const int per = NP * nv;
     const uint32_t mper = ((1u << 20) + per - 1) / per, mnv = ((1u << 20) + nv - 1) / nv;   // k / per, r / nv by multiplication (exact below 2^20 / divisor)
     for (int k = lane; k < NS * per; k += W) {
@@ -450,17 +491,11 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
     const T* qrow = U + (size_t)slot * Sq;
     const T* eprow = qrow + nq;
     const int32_t* dofqadr = P.i(h.off_dofqadr);
-    for (int p = 0; p < NP; ++p) {
-      const float* pr = P.f(h.off_posture) + p * (2 + nv);
-      if (pr[1] != 0.f) {
-        T s = T(0);
-        for (int d = 0; d < nv; ++d) { T v = T(pr[2 + d]) * T(pr[0]) * eprow[p * nv + d]; s += v * v; }
-        mu += T(pr[1]) * s;
-      }
-    }
+    if (NP > 0) mu = k2t_posture_lm<T>(P, eprow, mu);
     for (int d = l; d < nv; d += G) {
       const int u = umap[d];
       T hd = mu, cd = T(0);
+      #pragma unroll 1
       for (int p = 0; p < NP; ++p) {
         const float* pr = P.f(h.off_posture) + p * (2 + nv);
         const T wgt = T(pr[2 + d]);
@@ -508,8 +543,10 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   constexpr int IB = sizeof(M) == 8 ? 6 : 5;                       // index bits in the packed (value, index) keys
   constexpr uint32_t KEYV = 0x7fffffffu & ~((1u << IB) - 1u), KEYI = (1u << IB) - 1u;
   M lom = M(0), upm = M(0);
-  bool guessed = false;
-  const bool guess = sizeof(T) == 8 && h.k2_sweeps > 0 && nf < nu;   // fp64 only: fp32's gradient tolerance (1e-4) would accept a wrongly clamped dof
+  // STEP: when nf == nu nothing is guessed, but the loop below does not run either, and the warm-mask decode would find no
+  // finite bound to put a dof on: lom = upm = 0 all the same.
+  bool guessed = STEP;
+  const bool guess = sizeof(T) == 8 && (STEP || h.k2_sweeps > 0) && nf < nu;   // fp64 only: fp32's gradient tolerance (1e-4) would accept a wrongly clamped dof
   if (guess) {
     // Starting point of the guess: zero, or -- inside a rollout, from its second step on -- the previous step's dq (still
     // in a.dq; the warm-state bytes carry a marker once this kernel has written it), clipped to this step's box.
@@ -525,10 +562,10 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
       BIK_SYNCWARP();
     }
     k2t_pgs_guess<T, G, NS, M>(Hp, c, lo, hi, vs, rhsrow, Lp + tri(nu - 1) * NS, nu, nf, l, h.k2_sweeps, have_prev, &lom, &upm);   // scratch: free strips of the factor
-    guessed = h.k2_rule != 0;
+    guessed = STEP || h.k2_rule != 0;
     for (int k = nf + l; k < nu; k += G) xf[k * NS] = vs[k * NS];   // the Gauss-Seidel iterate is feasible: it is where the active-set method starts
     BIK_SYNCWARP();
-  } else if (a.warm) {   // (warp-uniform branch)
+  } else if (!STEP && a.warm) {   // (warp-uniform branch)
     if (live) {
       const signed char* wm = a.warm + b * nu;
       for (int i = nf; i < nu; ++i) {
@@ -655,7 +692,7 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   if (live && l == 0) {
     if (a.status) a.status[b] |= st;
     if (a.iters) a.iters[b] = it;
-    if (a.warm) { signed char* wm = a.warm + b * nu; for (int i = 0; i < nu; ++i) wm[i] = (signed char)((((lom >> i) & M(1)) ? 1 : (((upm >> i) & M(1)) ? 2 : 0)) | 4); }   // +4: a.dq holds this step's result
+    if (a.warm) k2t_store_warm<M>(a.warm + b * nu, nu, lom, upm);
   }
   BIK_SYNCWARP();
   // ---- q <- q (+) dq (Configuration.integrate_inplace, configuration.py:228-236): the lanes of a group take the nodes in turn ----
@@ -665,11 +702,12 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
     const int32_t* dofqadr = P.i(h.off_dofqadr);
     const uint32_t mnv = ((1u << 20) + nv - 1) / nv;
     auto sweep = [&](auto* qg, const auto* dg) {
+      #pragma unroll 1
       for (int k = lane; k < cnt * nv; k += W) {
         const int i = (int)(((uint32_t)k * mnv) >> 20), d = k - i * nv, qa = dofqadr[d];
         if (qa >= 0 && !(a.skip && a.skip[b0 + i])) qg[(b0 + i) * nq + qa] += dg[(b0 + i) * nv + d];
       }
-      if (live) for (int nn = l; nn < h.nnode; nn += G) { const NodeRec& r = P.node(nn); if (r.type == JNT_FREE || r.type == JNT_BALL) integrate_node(r, qg + b * nq, dg + b * nv); }
+      if (live) for (int nn = l; nn < h.nnode; nn += G) { const NodeRec& r = P.node(nn); if (r.type == JNT_FREE || r.type == JNT_BALL) k2t_integrate_quat_node(r, qg + b * nq, dg + b * nv); }
     };
     if (F32IO || !io64) sweep(reinterpret_cast<float*>(const_cast<void*>(a.q)), reinterpret_cast<const float*>(a.dq));   // fp32 buffers: fp32 arithmetic, as bik_integrate
     else sweep(reinterpret_cast<double*>(const_cast<void*>(a.q)), reinterpret_cast<const double*>(a.dq));
