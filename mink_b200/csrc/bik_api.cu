@@ -207,17 +207,13 @@ extern "C" int bik_problem_create(const bik_model* model, const bik_task_desc* t
   if (!build_image(model->hm, tasks, ntasks, limits, nlimits, model->G, &p->image, &err)) { delete p; return bik_fail(BIK_ERR_UNSUPPORTED, err); }
   {  // launch-independent solver knob kept in the image header so that every K2 entry point sees it
     PHeader* hh = reinterpret_cast<PHeader*>(p->image.data());
-    hh->k2_sweeps = std::max(0, std::min(16, env_int("BIK_K2_SWEEPS", hh->k2_sweeps)));
-    hh->k2_rule = env_int("BIK_K2_RULE", hh->k2_rule) != 0;
+    hh->k2_sweeps = std::max(1, std::min(16, env_int("BIK_K2_SWEEPS", hh->k2_sweeps)));
   }
   memcpy(&p->h, p->image.data(), sizeof(PHeader));
-  const char* prec = getenv("BIK_SOLVE_PRECISION");
-  p->solve_double = !(prec && (std::string(prec) == "f32" || std::string(prec) == "float"));
   const char* path = getenv("BIK_K2_PATH");
   p->k2_general = path && (std::string(path) == "dense" || std::string(path) == "general");
   p->k2_group = env_int("BIK_K2_GROUP", p->h.nu > 8 ? 8 : 4) == 8 ? 8 : 4;
   p->k2_warps = env_int("BIK_K2_WARPS", 8);
-  p->k2_lanes = env_int("BIK_K2_LANES", 0);
   p->k2_dynamic = env_int("BIK_K2_DYNAMIC", 1) != 0;
   if (p->k2_warps != 1 && p->k2_warps != 2 && p->k2_warps != 4 && p->k2_warps != 8) p->k2_warps = 8;
   const char* k1p = getenv("BIK_K1_PRECISION");
@@ -569,7 +565,7 @@ extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* 
   std::string d = "k1: " + std::to_string(h.G) + " lanes/instance, " + std::to_string(h.nneeded) + "/" + std::to_string(h.nnode) + " nodes visited, " +
                   (k1_double(p, damping, false) ? "f64" : "f32") + " for fp32 callers; nv=" + std::to_string(h.nv) + " coupled=" + std::to_string(h.nu) +
                   " (unbounded, eliminated once: " + std::to_string(grp ? h.nfree : 0) + ") rows=" + std::to_string(h.K) + " pairs=" + std::to_string(h.npairs) +
-                  " packed=" + std::to_string(h.pk_stride) + "; k2: " + k2 + ((p->solve_double || h.nu > K2T_NMAX) ? " f64" : " f32");
+                  " packed=" + std::to_string(h.pk_stride) + "; k2: " + k2 + " f64";
   if (buf && cap) { size_t n = d.size() < cap - 1 ? d.size() : cap - 1; memcpy(buf, d.c_str(), n); buf[n] = 0; }
   return (int)d.size();
 }

@@ -341,7 +341,7 @@ inline bool build_image(const HostModel& m, const bik_task_desc* tasks, int ntas
     // minimised over them in closed form once, the active-set iterations run on the rest (bik_k2t.h).  Only a prefix
     // of the (ascending) coupled list qualifies, which is where MuJoCo's dof order puts a floating base.
     H.nfree = 0;
-    H.k2_sweeps = 3; H.k2_rule = 1;   // BIK_K2_SWEEPS / BIK_K2_RULE override (bik_problem_create)
+    H.k2_sweeps = 3;   // BIK_K2_SWEEPS overrides it (bik_problem_create)
     if (H.npairs == 0) {
       auto bounded = [&](int d) {
         if (b.f(H.off_vmax)[d] < INF) return true;

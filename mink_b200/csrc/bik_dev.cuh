@@ -2,8 +2,8 @@
 // structs behind the C ABI and the launcher entry points each .cu exports to bik_api.cu.
 //
 //   bik_k1.cu   k1_kernel<T,G> (FK + task rows + collision rows + check_limits), fk_kernel<T,G> (Configuration API)
-//   bik_k2.cu   k2_kernel<T,W,SLOTS>  (general QP path: W = 8 / 16 / 32 lanes per problem)
-//   bik_k2t.cu  k2t_kernel<T,G,M>   (small-group QP path: G lanes per problem, 32- or 64-bit active-set masks)
+//   bik_k2.cu   k2_kernel<W,SLOTS>  (general QP path, fp64: W = 8 / 16 / 32 lanes per problem)
+//   bik_k2t.cu  k2t_kernel<double,G,256,M,..>  (small-group QP path, fp64: G lanes per problem, 32- or 64-bit active-set masks)
 //   bik_api.cu  C ABI (include/bik.h), workspace, bik_step / bik_converge / bik_step_host, small tiled kernels
 //
 // There is no CPU fallback in this library: without a CUDA device every entry point fails.
@@ -74,11 +74,9 @@ struct bik_problem {
   std::vector<uint32_t> image;
   uint32_t* d_image = nullptr;
   bik::PHeader h;
-  int solve_double = 1;   // BIK_SOLVE_PRECISION=f32 selects the fp32 instantiations of K2
   int k2_general = 0;     // BIK_K2_PATH=dense: every problem takes the general warp-per-problem path
   int k2_group = 8;       // lanes per problem on the small-group path (BIK_K2_GROUP = 4 | 8)
   int k2_warps = 8;       // warps per CTA of the general K2 kernel (BIK_K2_WARPS)
-  int k2_lanes = 0;       // lanes per problem of the general K2 kernel (BIK_K2_LANES = 8 | 16 | 32; 0: by the number of coupled dofs)
   int k2_dynamic = 1;     // BIK_K2_DYNAMIC=0: static tile assignment in the small-group K2
   int k1_prec = 0;        // BIK_K1_PRECISION: 0 auto (by conditioning estimate), 1 f32, 2 f64
   double max_cost2 = 0, min_post2 = 0;   // largest squared task cost / smallest squared posture cost over the coupled, bounded dofs

@@ -5,7 +5,7 @@ using namespace bik;
 
 // W lanes per problem (32 / W problems per warp): 8 or 16 when the augmented factor (coupled dofs + right-hand side) has at most
 // that many rows -- a 6-dof arm with collision rows leaves 26 of 32 lanes idle with a warp per problem.
-template <typename T, int W, int SLOTS>
+template <int W, int SLOTS>
 __global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2Args a) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ __align__(8) uint64_t bar;
@@ -15,39 +15,33 @@ __global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gi
   constexpr int PPW = 32 / W;
   const int warp = threadIdx.x >> 5, lane32 = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   const int grp = lane32 / W, lane = lane32 % W;
-  char* wsm = reinterpret_cast<char*>(smem + words) + (size_t)(warp * PPW + grp) * k2_warp_bytes(P.h(), sizeof(T));
+  char* wsm = reinterpret_cast<char*>(smem + words) + (size_t)(warp * PPW + grp) * k2_warp_bytes(P.h(), sizeof(double));
   for (long long b = (long long)(blockIdx.x * nwarps + warp) * PPW + grp; b < a.B; b += (long long)gridDim.x * nwarps * PPW)
-    k2_warp<T, W, SLOTS>(P, a, (int)b, wsm, lane);
+    k2_warp<double, W, SLOTS>(P, a, (int)b, wsm, lane);
 }
 
-template <typename T, int W, int SLOTS>
+template <int W, int SLOTS>
 static int launch_k2(const bik_problem* p, const K2Args& a, cudaStream_t st) {
   const PHeader& h = p->h;
   constexpr int PPW = 32 / W;
   int NW = p->k2_warps;
-  auto need = [&](int nw) { return (size_t)h.words32 * 4 + (size_t)nw * PPW * k2_warp_bytes(h, sizeof(T)); };
+  auto need = [&](int nw) { return (size_t)h.words32 * 4 + (size_t)nw * PPW * k2_warp_bytes(h, sizeof(double)); };
   while (NW > 1 && (int)need(NW) > p->model->max_smem) NW >>= 1;
   size_t smem = need(NW);
   int grid = 1;
   const long long per_cta = (long long)NW * PPW;
-  int rc = bik_launch_geometry((const void*)k2_kernel<T, W, SLOTS>, p->model, smem, 32 * NW, ((long long)a.B + per_cta - 1) / per_cta, &grid);
+  int rc = bik_launch_geometry((const void*)k2_kernel<W, SLOTS>, p->model, smem, 32 * NW, ((long long)a.B + per_cta - 1) / per_cta, &grid);
   if (rc) return rc;
-  k2_kernel<T, W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
+  k2_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
-template <typename T>
-static int dispatch_k2_slots(const bik_problem* p, const K2Args& a, cudaStream_t st) {
-  const int rows = p->h.nu + 1;           // rows of the augmented factor (coupled dofs + rhs): lanes x SLOTS must cover them
-  const int lanes = p->k2_lanes;          // BIK_K2_LANES: 0 = by size
-  if ((lanes == 8 || lanes == 0) && rows <= 8) return launch_k2<T, 8, 1>(p, a, st);
-  if ((lanes == 16 || lanes == 0) && rows <= 16) return launch_k2<T, 16, 1>(p, a, st);
-  const int slots = (rows + 31) / 32;
-  if (slots <= 1) return launch_k2<T, 32, 1>(p, a, st);
-  if (slots == 2) return launch_k2<T, 32, 2>(p, a, st);
-  return launch_k2<T, 32, 3>(p, a, st);
-}
 int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) {
-  const bool dbl = p->solve_double || a.io64 || a.pk64 || a.gc64 || a.dense64;
-  return dbl ? dispatch_k2_slots<double>(p, a, st) : dispatch_k2_slots<float>(p, a, st);
+  const int rows = p->h.nu + 1;           // rows of the augmented factor (coupled dofs + rhs): lanes x SLOTS must cover them
+  if (rows <= 8) return launch_k2<8, 1>(p, a, st);
+  if (rows <= 16) return launch_k2<16, 1>(p, a, st);
+  const int slots = (rows + 31) / 32;
+  if (slots <= 1) return launch_k2<32, 1>(p, a, st);
+  if (slots == 2) return launch_k2<32, 2>(p, a, st);
+  return launch_k2<32, 3>(p, a, st);
 }

@@ -105,19 +105,11 @@ BIK_HD int k2_warp_bytes(const PHeader& h, int ts) {
   return (bytes + 15) & ~15;
 }
 
-template <typename T> BIK_HD T bik_rsqrt(T x);
-template <> BIK_HD float bik_rsqrt<float>(float x) {
-#if defined(__CUDA_ARCH__)
-  return rsqrtf(x);
-#else
-  return 1.0f / sqrtf(x);
-#endif
-}
-template <> BIK_HD double bik_rsqrt<double>(double x) {
+template <typename T> BIK_HD T bik_rsqrt(T x) {
 #if defined(__CUDA_ARCH__)
   return rsqrt(x);
 #else
-  return 1.0 / sqrt(x);
+  return T(1) / sqrt(x);
 #endif
 }
 
@@ -447,7 +439,7 @@ BIK_NOINLINE int k2_general_rows(const K2Ws<T> w, const K2Args& a, long long gba
       // with h = 0: pairs at the minimum distance).  A relative shift of the diagonal turns the multipliers of such a family
       // into the minimum-norm split of their common multiplier: the signs stay meaningful and the method proceeds instead of
       // cycling (ALOHA with 1 104 pairs, 2 048 sampled instances: 89 flagged without the shift, 0 with it).
-      const T sjj = S[j * mg + j] * (T(1) + T(sizeof(T) == 8 ? 1e-12 : 1e-5));
+      const T sjj = S[j * mg + j] * (T(1) + T(1e-12));
       T d = sjj; for (int k = 0; k < j; ++k) d -= S[j * mg + k] * S[j * mg + k];
       if (!(d > T(1e-14) * sjj)) bad = 1;   // the active rows are (numerically) dependent beyond what the shift absorbs
       d = bik_sqrt<T>(d > T(0) ? d : T(1e-30)); S[j * mg + j] = d;
@@ -462,9 +454,7 @@ BIK_NOINLINE int k2_general_rows(const K2Ws<T> w, const K2Args& a, long long gba
   return warp_max_i<W>(bad);
 }
 
-template <typename T> struct K2Tol;
-template <> struct K2Tol<double> { static BIK_HD double x() { return 1e-12; } static BIK_HD double g() { return 1e-9; } };
-template <> struct K2Tol<float> { static BIK_HD float x() { return 1e-7f; } static BIK_HD float g() { return 1e-4f; } };
+template <typename T> struct K2Tol { static BIK_HD T x() { return T(1e-12); } static BIK_HD T g() { return T(1e-9); } };   // fp64 solve tolerances
 
 // Minimiser of the QP on the working set (w.st: 0 free / 1 at lower / 2 at upper; w.gst: active general rows) into w.x,
 // multipliers of the active general rows into w.lam.  Returns status bits (4: factorisation broke down, 2: more than

@@ -6,14 +6,17 @@
 // CTA to leave (sched[1] counts them) rewinds the counter for the next launch on the stream.
 //
 // The kernel is bound by instruction issue and fetch, so its code size is part of its speed.  bik_step, bik_step_host and
-// bik_converge launch a STEP instantiation (fp64 solve, fp32 buffers, packed rows, default solver settings) that leaves out
-// the code of the other forms, keeps one-off work out of line and does not unroll the solver loops: 9 216 SASS instructions
-// on sm_90a for G = 8 instead of 17 592, and K2 in the G1 step 0.60 ms instead of 0.78 ms on one H100 80GB HBM3 (SXM, 700 W
-// power limit).  tests/test_k2_code_size_cpu.py keeps it that size.
+// bik_converge launch a STEP instantiation (fp32 buffers, packed rows) that leaves out the dense-row staging, keeps one-off
+// work out of line and does not unroll the solver loops: 9 216 SASS instructions on sm_90a for G = 8 instead of 17 592, and
+// K2 in the G1 step 0.60 ms instead of 0.78 ms on one H100 80GB HBM3 (SXM, 700 W power limit).
+// tests/test_k2_code_size_cpu.py keeps it that size.
 #include "bik_dev.cuh"
 
 using namespace bik;
 
+constexpr int K2T_MAXT = 256;   // threads per CTA at most; two CTAs per SM
+
+// Launched as k2t_kernel<double, G, K2T_MAXT, ...> only; T and MAXT stay in the template, and so in the kernel's symbol.
 template <typename T, int G, int MAXT, typename M, bool F32IO, bool STEP>
 __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_kernel(const uint32_t* __restrict__ gimage, int warp_bytes, K2Args a, unsigned int* sched) {
   extern __shared__ __align__(16) uint32_t smem[];
@@ -23,7 +26,7 @@ __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_kernel(const uint32_t* _
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   char* wsm = reinterpret_cast<char*>(smem) + (size_t)warp * warp_bytes;
   const long long ntiles = ((long long)a.B + NS - 1) / NS;
-  const int St = k2t_task_tile_words(P), uw = k2t_union_words(P, sizeof(T));
+  const int St = k2t_task_tile_words(P), uw = k2t_union_words(P);
   if (sched) {
     for (;;) {
       unsigned int t = 0;
@@ -40,63 +43,60 @@ __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_kernel(const uint32_t* _
     k2t_warp_tile<T, G, NS, M, F32IO, STEP>(P, a, tile * NS, wsm, lane, St, uw);
 }
 
-template <typename T, int G, typename M, bool F32IO, bool STEP>
-static int launch_k2t_io(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
-  constexpr int NS = 32 / G, MAXT = sizeof(T) == 8 ? 256 : 512;
-  PView P{p->image.data()};
-  const size_t wb = (size_t)k2t_warp_bytes(P, sizeof(T), NS);
-  int NW = MAXT / 32;
+// warps per CTA: as many as shared memory holds, at most K2T_MAXT / 32
+static int k2t_warps(const bik_problem* p, size_t wb) {
+  int NW = K2T_MAXT / 32;
   while (NW > 1 && NW * wb > (size_t)p->model->max_smem) --NW;
+  return NW;
+}
+template <int G, typename M, bool F32IO, bool STEP>
+static int launch_k2t_io(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
+  constexpr int NS = 32 / G;
+  PView P{p->image.data()};
+  const size_t wb = (size_t)k2t_warp_bytes(P, sizeof(double), NS);
+  const int NW = k2t_warps(p, wb);
   const size_t smem = NW * wb;
   int grid = 1;
   long long tiles = ((long long)a.B + NS - 1) / NS;
-  int rc = bik_launch_geometry((const void*)k2t_kernel<T, G, MAXT, M, F32IO, STEP>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
+  int rc = bik_launch_geometry((const void*)k2t_kernel<double, G, K2T_MAXT, M, F32IO, STEP>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
   if (rc) return rc;
-  k2t_kernel<T, G, MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
+  k2t_kernel<double, G, K2T_MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
-template <typename T, int G, typename M>
+template <int G, typename M>
 static int launch_k2t(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
-  if (sizeof(T) == 4 || !(a.io64 || a.pk64 || a.dense64)) {   // fp32 buffers everywhere
-    // the step's form (packed rows from K1, active-set guess, primal pivoting rule): the fp64 solve without the other forms' code
-    const bool step = sizeof(T) == 8 && a.pk && !a.ep && p->h.k2_sweeps > 0 && p->h.k2_rule == 1;
-    if (step) return launch_k2t_io<T, G, M, true, sizeof(T) == 8>(p, a, sched, st);
-    return launch_k2t_io<T, G, M, true, false>(p, a, sched, st);
-  }
-  return launch_k2t_io<T, G, M, sizeof(T) == 4, false>(p, a, sched, st);
+  if (a.io64 || a.pk64 || a.dense64) return launch_k2t_io<G, M, false, false>(p, a, sched, st);
+  // fp32 buffers everywhere; packed rows from K1 are the step's form
+  return a.pk ? launch_k2t_io<G, M, true, true>(p, a, sched, st) : launch_k2t_io<G, M, true, false>(p, a, sched, st);
 }
 static int group_of(const bik_problem* p) { return (p->h.nu > K2T_NMAX || p->k2_group == 8) ? 8 : 4; }
-static bool use_double(const bik_problem* p, const K2Args& a) { return p->solve_double || a.io64 || a.pk64 || a.dense64 || p->h.nu > K2T_NMAX; }
 
 bool bik_k2_group_applies(const bik_problem* p) {
   const PHeader& h = p->h;
   if (p->k2_general || h.npairs != 0 || h.nu < 1 || h.nu > K2T_NMAX_WIDE) return false;
   PView P{p->image.data()};
-  const int ts = (p->solve_double || h.nu > K2T_NMAX) ? 8 : 4;
-  return k2t_warp_bytes(P, ts, 32 / group_of(p)) <= p->model->max_smem;
+  return k2t_warp_bytes(P, sizeof(double), 32 / group_of(p)) <= p->model->max_smem;
 }
 long long bik_k2_group_wave(const bik_problem* p) {
   if (!bik_k2_group_applies(p)) return 0;
   PView P{p->image.data()};
-  const int G = group_of(p), NS = 32 / G, ts = (p->solve_double || p->h.nu > K2T_NMAX) ? 8 : 4, maxt = ts == 8 ? 256 : 512;
-  const size_t wb = (size_t)k2t_warp_bytes(P, ts, NS);
-  int NW = maxt / 32;
-  while (NW > 1 && NW * wb > (size_t)p->model->max_smem) --NW;
+  const int NS = 32 / group_of(p);
+  const size_t wb = (size_t)k2t_warp_bytes(P, sizeof(double), NS);
+  const int NW = k2t_warps(p, wb);
   int per_sm = (int)((size_t)p->model->max_smem / (NW * wb + 1024));   // estimate; only used to size chunks
   if (per_sm < 1) per_sm = 1;
   return (long long)p->model->nsm * per_sm * NW * NS;
 }
 int bik_launch_k2_group(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
-  if (p->h.nu > K2T_NMAX) return launch_k2t<double, 8, uint64_t>(p, a, sched, st);   // wide: 64-bit active-set masks
-  if (use_double(p, a)) return group_of(p) == 8 ? launch_k2t<double, 8, uint32_t>(p, a, sched, st) : launch_k2t<double, 4, uint32_t>(p, a, sched, st);
-  return group_of(p) == 8 ? launch_k2t<float, 8, uint32_t>(p, a, sched, st) : launch_k2t<float, 4, uint32_t>(p, a, sched, st);
+  if (p->h.nu > K2T_NMAX) return launch_k2t<8, uint64_t>(p, a, sched, st);   // wide: 64-bit active-set masks
+  return group_of(p) == 8 ? launch_k2t<8, uint32_t>(p, a, sched, st) : launch_k2t<4, uint32_t>(p, a, sched, st);
 }
 const char* bik_k2_describe(const bik_problem* p, char* buf, size_t cap) {
   if (bik_k2_group_applies(p)) snprintf(buf, cap, "small-group G=%d%s", group_of(p), p->h.nu > K2T_NMAX ? " (64-bit masks)" : "");
   else {
-    const int rows = p->h.nu + 1, want = p->k2_lanes;
-    const int lanes = ((want == 8 || want == 0) && rows <= 8) ? 8 : (((want == 16 || want == 0) && rows <= 16) ? 16 : 32);
+    const int rows = p->h.nu + 1;
+    const int lanes = rows <= 8 ? 8 : (rows <= 16 ? 16 : 32);
     if (lanes == 32) snprintf(buf, cap, "general warp-per-problem");
     else snprintf(buf, cap, "general %d-lanes-per-problem", lanes);
   }

@@ -1,11 +1,11 @@
 // bik_k2t.h -- K2, small-group path: the same QP as bik_k2.h (same objective, same box, same tolerances, same optimum),
-// laid out for coupled blocks of up to 32 dofs.
+// laid out for coupled blocks of up to 64 dofs (32-bit active-set masks up to 32, 64-bit ones beyond).
 //
 // Why: with a whole warp per instance the 18-dof coupled block of the G1 configuration keeps half the
 // lanes idle and spends most instructions on run-time index arithmetic, shuffles and barriers
 // (14 k warp-instructions per instance, ~45 k cycles per pivoting iteration).  Here G adjacent lanes
-// (4 or 8) share one problem, so a warp carries NS = 32/G problems; the loops are compact run-time loops
-// over shared memory so that a whole pivoting iteration stays resident in the instruction cache:
+// (4 or 8) share one problem, so a warp carries NS = 32/G problems; the solve is in fp64, and its loops are compact
+// run-time loops over shared memory so that a whole pivoting iteration stays resident in the instruction cache:
 //
 //   * per-instance vectors and packed triangles live in shared memory, word w of slot s at [w*NS + s]
 //     (the G lanes of a group broadcast-read one address; the NS groups read one 8*NS-byte segment);
@@ -18,8 +18,7 @@
 //     previous step's dq; a primal active-set method then starts from that feasible point: every iteration
 //     refactors the pivoted block with clamped dofs turned into identity rows/columns (masked loads), so every
 //     group executes the same instruction stream whatever its active set is and groups never diverge; a group
-//     that has converged idles until its warp is done.  Without a guess (fp32 instantiation, BIK_K2_SWEEPS=0)
-//     the iterations are block principal pivoting as in bik_k2.h;
+//     that has converged idles until its warp is done;
 //   * the factorisation is left-looking by blocks of G rows: lane l owns row i0+l, finished rows are
 //     broadcast-read from shared memory, the right-hand side rides along as the last row (forward
 //     substitution for free), diagonals are kept as reciprocal square roots, entries masked out by the
@@ -54,17 +53,9 @@ BIK_HD int bik_popc(uint32_t v) {
   return __builtin_popcount(v);
 #endif
 }
-BIK_HD int bik_clz(uint32_t v) {   // v != 0
-#if defined(__CUDA_ARCH__)
-  return __clz((int)v);
-#else
-  return __builtin_clz(v);
-#endif
-}
+BIK_HD int bik_popc(uint64_t v) { return bik_popc((uint32_t)v) + bik_popc((uint32_t)(v >> 32)); }
 
 enum { K2T_NMAX = 32, K2T_NMAX_WIDE = 64 };   // 32-bit active-set masks by default, 64-bit in the wide instantiation
-BIK_HD int bik_popc(uint64_t v) { return bik_popc((uint32_t)v) + bik_popc((uint32_t)(v >> 32)); }
-BIK_HD int bik_clz(uint64_t v) { return (uint32_t)(v >> 32) ? bik_clz((uint32_t)(v >> 32)) : 32 + bik_clz((uint32_t)v); }   // v != 0  // largest coupled block this path takes (active sets are 32-bit masks)
 
 // ---- group reductions over G adjacent lanes (every lane of the warp must call them) --------------------
 template <int G> BIK_HD int grp_or(int v) {
@@ -111,18 +102,17 @@ BIK_HD int k2t_task_tile_words(const PView& P) {  // widest task tile, in T word
   if (h.C > 0) { int ne = 3 * h.com_ncols + 3; m = ne > m ? ne : m; }
   return m | 1;
 }
-BIK_HD int k2t_union_words(const PView& P, int ts) {
+BIK_HD int k2t_union_words(const PView& P) {
   const PHeader& h = P.h();
   int u = tri(h.nu + 1);
   int t = k2t_task_tile_words(P);
   u = t > u ? t : u;
   int fw = (h.nq + h.P * h.nv) | 1;   // q (+ dense posture errors) of one instance, as T
-  (void)ts;
   return fw > u ? fw : u;
 }
-BIK_HD int k2t_slot_T_words(const PView& P, int ts) { return tri(P.h().nu) + k2t_union_words(P, ts) + 3 * P.h().nu; }
-BIK_HD int k2t_slot_bytes(const PView& P, int ts) { return k2t_slot_T_words(P, ts) * ts + 2 * P.h().nu * 4; }
-BIK_HD int k2t_warp_bytes(const PView& P, int ts, int NS) { return (NS * k2t_slot_bytes(P, ts) + 15) & ~15; }
+BIK_HD int k2t_slot_T_words(const PView& P) { return tri(P.h().nu) + k2t_union_words(P) + 3 * P.h().nu; }
+BIK_HD int k2t_slot_bytes(const PView& P, int ts) { return k2t_slot_T_words(P) * ts + 2 * P.h().nu * 4; }
+BIK_HD int k2t_warp_bytes(const PView& P, int ts, int NS) { return (NS * k2t_slot_bytes(P, ts) + 15) & ~15; }   // ts: sizeof(T)
 
 // ---- staging (warp-cooperative, W lanes, NS instances) -------------------------------------------------
 // One task's weighted block, column-major like K1's packed record:
@@ -213,18 +203,8 @@ BIK_HD void k2t_task_accumulate(const T* tr, int nr, int nc, const int32_t* cols
 // the assembly carries `#pragma unroll 1`: unrolled by the compiler they made the step's kernel 17.6 k SASS instructions on
 // sm_90a, and even the factor's and the assembly's dot loops alone cost 6 % of K2's time in the G1 step on an H100 --------
 // Dot product of row i of the symmetric packed matrix with a vector (both slot-strided in shared memory).
-#ifdef BIK_K2T_NOINLINE_ROWDOT
-#define BIK_K2T_ROWDOT_ATTR BIK_NOINLINE
-#else
-#define BIK_K2T_ROWDOT_ATTR BIK_HD
-#endif
-#ifdef BIK_K2T_INLINE_FACTOR
-#define BIK_K2T_FACTOR_ATTR BIK_HD
-#else
-#define BIK_K2T_FACTOR_ATTR BIK_NOINLINE
-#endif
 template <typename T, int NS>
-BIK_K2T_ROWDOT_ATTR T k2t_row_dot(const T* __restrict__ Hp, const T* __restrict__ v, int i, int nu, int k0 = 0) {   // sum over m in [k0, nu), i >= k0
+BIK_HD T k2t_row_dot(const T* __restrict__ Hp, const T* __restrict__ v, int i, int nu, int k0 = 0) {   // sum over m in [k0, nu), i >= k0
   const T* row = Hp + (tri(i) + k0) * NS;
   const T* pv = v + k0 * NS;
   T a0 = T(0), a1 = T(0);
@@ -248,7 +228,7 @@ BIK_K2T_ROWDOT_ATTR T k2t_row_dot(const T* __restrict__ Hp, const T* __restrict_
 //             complement of the leading block; columns < nf of Lp are left alone.
 // Every lane of the warp must call it (it contains warp barriers).
 template <typename T, int G, int NS, typename M>
-BIK_K2T_FACTOR_ATTR int k2t_factor(const T* __restrict__ Hp, T* __restrict__ Lp, int nu, M act, int l, int kb, int ke) {
+BIK_NOINLINE int k2t_factor(const T* __restrict__ Hp, T* __restrict__ Lp, int nu, M act, int l, int kb, int ke) {
   int bad = 0;
   T* const rhsrow = Lp + tri(nu) * NS;
   // Row blocks are aligned to the END of the system (rows kb..nu): the last rows are the expensive ones (cost ~ i^2),
@@ -329,7 +309,7 @@ BIK_HD void k2t_backsub_cross(T* __restrict__ Lp, int nu, int l, const T* __rest
 //   x_i <- clip(-(c_i + sum_{m != i} S_im x_m) / S_ii, lo_i, hi_i),  i = k0 .. nu-1,  `sweeps` times from x = 0.
 // Every lane of a group computes x_i and records which bound it sits on; the G lanes split the update of the residual
 // (two warp barriers per row).  The guess only has to be
-// close: block principal pivoting below starts from it and still ends at the exact optimum.  After the free-joint
+// close: the primal active-set method below starts from it and still ends at the exact optimum.  After the free-joint
 // dofs have been eliminated the remaining block is strongly diagonally dominant per limb, and three sweeps cut the
 // pivoting iterations of the G1 workload from 3.6 (4.5 for the slowest of the 4 problems in a warp) to 1.1 (1.4).
 // dinv and res (nu words each, slot-strided, entries [k0, nu) used) are scratch: 1 / S_ii and the residual c + S x.  At most `sweeps` sweeps; they stop as soon as a sweep leaves the set of
@@ -426,13 +406,12 @@ BIK_NOINLINE void k2t_store_warm(signed char* wm, int nu, M lom, M upm) {
 // F32IO (compile time): every caller buffer and the hand-off hold fp32 -- the batched fast path: the fp64 load / store /
 // integrate code is not even compiled in (it tripled the kernel's SASS and its instruction-fetch stalls).  Otherwise the
 // element types follow the run-time flags of K2Args.
-// STEP (compile time, with F32IO and T = double): the form bik_step / bik_step_host / bik_converge launch with the default
-// solver settings -- packed task rows (a.pk set, a.ep null), k2_sweeps > 0, k2_rule == 1.  Only the packed staging and the
-// guessed primal active-set loop are compiled in: no dense-row staging, no block-flip branch, no warm-mask decode.
+// STEP (compile time, with F32IO): the form bik_step / bik_step_host / bik_converge launch -- packed task rows (a.pk set,
+// a.ep null).  Only the packed staging is compiled in: no dense-row staging, no staging of dense posture errors.
 template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false>
 BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* wsm, int lane, int St = 0, int uw = 0) {
-  static_assert(!STEP || (F32IO && sizeof(T) == 8), "the step instantiation is fp64 on fp32 buffers");
-  if (St == 0) { St = k2t_task_tile_words(P); uw = k2t_union_words(P, sizeof(T)); }   // callers that loop over tiles pass them in
+  static_assert(!STEP || F32IO, "the step instantiation reads fp32 buffers");
+  if (St == 0) { St = k2t_task_tile_words(P); uw = k2t_union_words(P); }   // callers that loop over tiles pass them in
   const int io64 = F32IO ? 0 : a.io64, pk64 = F32IO ? 0 : a.pk64, dense64 = F32IO ? 0 : a.dense64;
   constexpr int W = G * NS;
   const PHeader& h = P.h();
@@ -522,11 +501,7 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   // active set, so they are produced once; the pivoting iterations then run on the Schur complement (nu - nf dofs:
   // 12 instead of 18 for the G1 configuration), and the leading part of x is recovered by continuing the last back
   // substitution.  With nf == 0 this block does nothing; with nf == nu (no bounded dof at all) it is the whole solve.
-#ifdef BIK_K2T_NO_ELIM   // A/B switch (tools/k2_variants.py): pivot on the whole coupled block as before
-  const int nf = 0;
-#else
   const int nf = h.nfree;
-#endif
   T* const rhsrow = Lp + tri(nu) * NS;
   if (nf > 0) {
     for (int k = l; k < nf; k += G) rhsrow[k * NS] = -c[k * NS];
@@ -537,16 +512,13 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
     BIK_SYNCWARP();
   }
 
-  // ---- block principal pivoting ----
-  const int MAXIT = 400, PATIENCE = 3;   // the primal active-set method needs ~20 at most; the block-pivoting branch (fp32, no guess) can need its slow fallback
+  // ---- active-set guess, then the primal active-set method ----
+  const int MAXIT = 400;   // the primal active-set method needs ~20 at most
   const T tolx = K2Tol<T>::x(), tolg = K2Tol<T>::g();
   constexpr int IB = sizeof(M) == 8 ? 6 : 5;                       // index bits in the packed (value, index) keys
   constexpr uint32_t KEYV = 0x7fffffffu & ~((1u << IB) - 1u), KEYI = (1u << IB) - 1u;
   M lom = M(0), upm = M(0);
-  // STEP: when nf == nu nothing is guessed, but the loop below does not run either, and the warm-mask decode would find no
-  // finite bound to put a dof on: lom = upm = 0 all the same.
-  bool guessed = STEP;
-  const bool guess = sizeof(T) == 8 && (STEP || h.k2_sweeps > 0) && nf < nu;   // fp64 only: fp32's gradient tolerance (1e-4) would accept a wrongly clamped dof
+  const bool guess = nf < nu;   // with nf == nu there is no bound to guess and the loop below does not run
   if (guess) {
     // Starting point of the guess: zero, or -- inside a rollout, from its second step on -- the previous step's dq (still
     // in a.dq; the warm-state bytes carry a marker once this kernel has written it), clipped to this step's box.
@@ -562,21 +534,10 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
       BIK_SYNCWARP();
     }
     k2t_pgs_guess<T, G, NS, M>(Hp, c, lo, hi, vs, rhsrow, Lp + tri(nu - 1) * NS, nu, nf, l, h.k2_sweeps, have_prev, &lom, &upm);   // scratch: free strips of the factor
-    guessed = STEP || h.k2_rule != 0;
     for (int k = nf + l; k < nu; k += G) xf[k * NS] = vs[k * NS];   // the Gauss-Seidel iterate is feasible: it is where the active-set method starts
     BIK_SYNCWARP();
-  } else if (!STEP && a.warm) {   // (warp-uniform branch)
-    if (live) {
-      const signed char* wm = a.warm + b * nu;
-      for (int i = nf; i < nu; ++i) {
-        int s0 = wm[i] & 3;
-        if (s0 == 1 && lo[i * NS] > -1e30f) lom |= M(1) << i;
-        else if (s0 == 2 && hi[i * NS] < 1e30f) upm |= M(1) << i;
-      }
-    }
   }
-  int best = nu + 1, patience = PATIENCE;
-  bool done = nf == nu;     // no bounded dof at all: the elimination above was the whole solve (one factorisation)
+  bool done = nf == nu;    // no bounded dof at all: the elimination above was the whole solve (one factorisation)
   int it = done ? 1 : 0;
   for (;;) {
     if (!BIK_WARP_ANY(!done && it < MAXIT)) break;
@@ -609,7 +570,7 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
         const bool above = !below && xi > bu + tolx * (T(1) + (bu < 0 ? -bu : bu));
         if (below) vlo |= bit;
         if (above) vup |= bit;
-        if (guessed && (below || above)) {   // how far the feasible iterate can move towards x before this bound stops it
+        if (below || above) {   // how far the feasible iterate can move towards x before this bound stops it
           const T xo = xf[k * NS], d = xi - xo;
           T al = d != T(0) ? ((below ? bl : bu) - xo) / d : T(0);
           al = al < T(0) ? T(0) : (al > T(1) ? T(1) : al);
@@ -630,48 +591,36 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
     worst = grp_max<G>(worst);
     T alpha = T(0), bound = T(0);
     int kb = 0;
-    if (guessed) {
-      blocking = -grp_max<G>(-blocking);
-      if (vlo | vup) {   // exact step length to the blocking bound (the key only ranked the candidates in fp32)
-        kb = blocking & (int)KEYI;
-        const T xo = xf[kb * NS], d = vs[kb * NS] - xo;
-        bound = ((vlo >> kb) & M(1)) ? T(lo[kb * NS]) : T(hi[kb * NS]);
-        alpha = d != T(0) ? (bound - xo) / d : T(0);
-        alpha = alpha < T(0) ? T(0) : (alpha > T(1) ? T(1) : alpha);
-      }
+    blocking = -grp_max<G>(-blocking);
+    if (vlo | vup) {   // exact step length to the blocking bound (the key only ranked the candidates in fp32)
+      kb = blocking & (int)KEYI;
+      const T xo = xf[kb * NS], d = vs[kb * NS] - xo;
+      bound = ((vlo >> kb) & M(1)) ? T(lo[kb * NS]) : T(hi[kb * NS]);
+      alpha = d != T(0) ? (bound - xo) / d : T(0);
+      alpha = alpha < T(0) ? T(0) : (alpha > T(1) ? T(1) : alpha);
     }
     BIK_SYNCWARP();   // every lane has read x (and the feasible iterate) before anything below or the next iteration overwrites them
     if (run) {
       ++it;
-      const M changed = vlo | vup | rel;
-      const int ninf = bik_popc(changed);
-      if (ninf == 0) done = true;
-      else if (guessed) {
-        // Primal active-set step from the feasible iterate xf (started at the Gauss-Seidel guess): block flips cycle on a few
-        // instances per thousand once a rollout is under way (the single-pivot fallback then runs out of its 60 iterations),
-        // and flipping every violated dof at once gives up monotone descent.  Here the objective decreases at every step,
-        // so the method terminates: move towards the subspace minimiser x until the first bound stops the move and clamp
-        // that dof; at a feasible subspace minimiser let go of the bound with the worst multiplier, or stop if there is none.
-        if (vlo | vup) {
-          for (int k = nf + l; k < nu; k += G) {
-            if (k == kb) xf[k * NS] = bound;
-            else if (!((act >> k) & M(1))) xf[k * NS] += alpha * (vs[k * NS] - xf[k * NS]);
-          }
-          const M bit = M(1) << kb;
-          if (vlo & bit) lom |= bit; else upm |= bit;
-        } else {
-          for (int k = nf + l; k < nu; k += G) xf[k * NS] = vs[k * NS];
-          const M bit = M(1) << (worst & (int)KEYI);
-          lom &= ~bit; upm &= ~bit;
+      // Primal active-set step from the feasible iterate xf (started at the Gauss-Seidel guess): block flips cycle on a few
+      // instances per thousand once a rollout is under way, and flipping every violated dof at once gives up monotone
+      // descent.  Here the objective decreases at every step, so the method terminates: move towards the subspace minimiser
+      // x until the first bound stops the move and clamp that dof; at a feasible subspace minimiser let go of the bound with
+      // the worst multiplier, or stop if there is none.
+      // (a population count, not a test of the mask: with the test, the 64-bit-mask step instantiation is laid out
+      // differently and g1_full's step was 0.5 % slower on one H100 80GB HBM3, SXM, 400 W power limit)
+      if (bik_popc(vlo | vup | rel) == 0) done = true;
+      else if (vlo | vup) {
+        for (int k = nf + l; k < nu; k += G) {
+          if (k == kb) xf[k * NS] = bound;
+          else if (!((act >> k) & M(1))) xf[k * NS] += alpha * (vs[k * NS] - xf[k * NS]);
         }
+        const M bit = M(1) << kb;
+        if (vlo & bit) lom |= bit; else upm |= bit;
       } else {
-        bool block;
-        if (ninf < best) { best = ninf; patience = PATIENCE; block = true; }
-        else if (patience > 0) { --patience; block = true; }
-        else block = false;
-        const M nlo = (lom & ~rel) | vlo, nup = (upm & ~rel) | vup;
-        if (block) { lom = nlo; upm = nup; }
-        else { const M bit = M(1) << ((int)(8 * sizeof(M)) - 1 - bik_clz(changed)); lom = (lom & ~bit) | (nlo & bit); upm = (upm & ~bit) | (nup & bit); }
+        for (int k = nf + l; k < nu; k += G) xf[k * NS] = vs[k * NS];
+        const M bit = M(1) << (worst & (int)KEYI);
+        lom &= ~bit; upm &= ~bit;
       }
     }
   }

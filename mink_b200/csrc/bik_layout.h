@@ -83,8 +83,8 @@ struct PHeader {  // all offsets in 32-bit words from the start of the image
   int32_t nneeded;      // nodes visited by the lane program (ancestors of frames / masses / collision geoms)
   int32_t nfree;        // leading coupled dofs (compact indices 0..nfree-1) without any finite bound: eliminated once by K2
   int32_t nslots;       // rows of the pose state = nodes visited by the lane program (nnode when slots are the identity)
-  int32_t k2_sweeps;    // projected Gauss-Seidel sweeps that guess the active set before K2's pivoting (0: cold start)
-  int32_t k2_rule;      // pivoting rule after a guess: 1 = clamp all violated dofs, release one bound at a time; 0 = block flips
+  int32_t k2_sweeps;    // projected Gauss-Seidel sweeps (1..16) that guess the active set before the small-group K2's pivoting
+  int32_t k2_rule;      // reserved: nothing reads it (the small-group K2 has one pivoting rule)
   int32_t words32;      // words the fp32 kernels stage (everything before the fp64 side tables)
   int32_t pk_stride;    // elements per instance of the packed K1 -> K2 record (multiple of 4)
   int32_t off_nodes64, off_frames64, off_qpos064, off_comnodes64, off_geoms64;   // fp64 side tables (word offsets, 8-byte aligned)

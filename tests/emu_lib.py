@@ -56,8 +56,8 @@ class Emu:
         names = ("nv", "nu", "nfree", "nnode", "nneeded", "nslots", "G", "nsteps", "pk_stride", "words32", "words")
         return dict(zip(names, (int(v) for v in out)))
 
-    def set_knobs(self, sweeps: int, rule: int):
-        lib().emu_set_knobs(self.h, int(sweeps), int(rule))
+    def set_knobs(self, sweeps: int):
+        lib().emu_set_knobs(self.h, int(sweeps))
 
     def fk_jac(self, q, ftgt=None, ptgt=None, ctgt=None, dt=1e-2, prec="f32", packed=False, check=False):
         """K1.  prec: "f32" (fp32 kernel, fp32 buffers), "f64" (fp64 kernel, fp64 buffers), "mixed" (fp64 kernel on fp32
@@ -86,9 +86,10 @@ class Emu:
 
     def solve(self, q, J, e, ep, Gc, hc, dt, damping, use_double=True, want_objective=False, io64=False, pk=None, ptgt=None,
               integrate=False, warm=None, skip=None, dq_inout=None):
-        """K2.  use_double: False/0 general fp32, True/1 general fp64, 3 small-group fp64, 4 small-group fp32, 8 small-group
-        fp64 with 64-bit masks.  Task rows dense (J, e, ep) or packed (pk; then the posture error comes from q and ptgt).
-        Returns (dq, status, iters, H, c, lo, hi) (+ q after integration when integrate=True)."""
+        """K2, fp64 solve.  use_double: True/1 general path, 3 small-group, 8 small-group with 64-bit masks (packed fp32
+        rows with fp32 I/O take the small-group step instantiation).  Task rows dense (J, e, ep) or packed (pk; then the
+        posture error comes from q and ptgt).  Returns (dq, status, iters, H, c, lo, hi) (+ q after integration when
+        integrate=True)."""
         s = self.spec
         path = int(use_double)
         tio = np.float64 if io64 else np.float32

@@ -34,9 +34,9 @@ extern "C" void emu_header(void* prob, int32_t* out) {
   out[0] = h.nv; out[1] = h.nu; out[2] = h.nfree; out[3] = h.nnode; out[4] = h.nneeded; out[5] = h.nslots; out[6] = h.G; out[7] = h.nsteps;
   out[8] = h.pk_stride; out[9] = h.words32; out[10] = h.words;
 }
-extern "C" void emu_set_knobs(void* prob, int sweeps, int rule) {   // what BIK_K2_SWEEPS / BIK_K2_RULE do in bik_problem_create
+extern "C" void emu_set_knobs(void* prob, int sweeps) {   // what BIK_K2_SWEEPS does in bik_problem_create
   PHeader* h = reinterpret_cast<PHeader*>(static_cast<EmuProblem*>(prob)->image.data());
-  h->k2_sweeps = sweeps; h->k2_rule = rule;
+  h->k2_sweeps = sweeps < 1 ? 1 : (sweeps > 16 ? 16 : sweeps);
 }
 extern "C" void emu_problem_destroy(void* p) { delete static_cast<EmuProblem*>(p); }
 
@@ -70,8 +70,17 @@ extern "C" int emu_fk_jac(void* prob, int B, int f64, const void* q, const void*
   return 0;
 }
 
-// K2.  path: 0 general fp32, 1 general fp64, 3 small-group fp64, 4 small-group fp32, 8 small-group fp64 with 64-bit masks.
+// K2 (fp64 solve).  path: 1 general, 3 small-group, 8 small-group with 64-bit masks.
 // Task rows: packed (pk, pk64) or dense (J, e, ep fp32; ep may be null with ptgt set).  io64: q / ptgt / dq are fp64.
+// Packed fp32 rows with fp32 I/O take the small-group step instantiation, as in bik_step.
+template <typename M>
+static void emu_k2t(const PView& P, const K2Args& a, int B, double* tw) {
+  const bool step = a.pk && !a.pk64 && !a.io64;
+  for (int b = 0; b < B; ++b) {
+    if (step) k2t_warp_tile<double, 1, 1, M, true, true>(P, a, b, tw, 0);
+    else k2t_warp_tile<double, 1, 1, M>(P, a, b, tw, 0);
+  }
+}
 extern "C" int emu_solve(void* prob, int B, int path, int io64, const void* q, const void* pk, int pk64, const float* J, const float* e, const float* ep,
                          const void* ptgt, int pbatched, const void* Gc, const void* hc, int gc64, double dt, double damping, void* dq,
                          int integrate, int32_t* status, int32_t* iters, double* H, double* c, void* lo, void* hi, signed char* warm,
@@ -83,22 +92,17 @@ extern "C" int emu_solve(void* prob, int B, int path, int io64, const void* q, c
   a.B = B; a.q = q; a.io64 = io64; a.pk = pk; a.pk64 = pk64; a.J = J; a.e = e; a.ep = ep; a.dense64 = 0; a.ptgt = ptgt; a.pbatched = pbatched;
   a.Gc = Gc; a.hc = hc; a.gc64 = gc64; a.dt = dt; a.damping = damping; a.dq = dq; a.integrate = integrate; a.status = status; a.iters = iters;
   a.Hout = H; a.cout = c; a.lo_out = lo; a.hi_out = hi; a.warm = warm; a.skip = skip;
-  if (path == 3 || path == 4 || path == 8) {
+  if (path == 3 || path == 8) {
     const int nmax = path == 8 ? K2T_NMAX_WIDE : K2T_NMAX;
     if (P.h().npairs != 0 || P.h().nu < 1 || P.h().nu > nmax) { g_err = "small-group path not applicable"; return -1; }
     std::vector<double> tw(k2t_warp_bytes(P, 8, 1) / 8 + 16);
-    for (int b = 0; b < B; ++b) {
-      if (path == 3) k2t_warp_tile<double, 1, 1>(P, a, b, tw.data(), 0);
-      else if (path == 4) k2t_warp_tile<float, 1, 1>(P, a, b, tw.data(), 0);
-      else k2t_warp_tile<double, 1, 1, uint64_t>(P, a, b, tw.data(), 0);
-    }
+    if (path == 3) emu_k2t<uint32_t>(P, a, B, tw.data());
+    else emu_k2t<uint64_t>(P, a, B, tw.data());
     return 0;
   }
+  if (path != 1) { g_err = "unknown K2 path " + std::to_string(path); return -1; }
   std::vector<double> wsm(k2_warp_bytes(P.h(), 8) / 8 + 16);
-  for (int b = 0; b < B; ++b) {
-    if (path) k2_warp<double, 1, 65>(P, a, b, wsm.data(), 0);
-    else k2_warp<float, 1, 65>(P, a, b, wsm.data(), 0);
-  }
+  for (int b = 0; b < B; ++b) k2_warp<double, 1, 65>(P, a, b, wsm.data(), 0);
   return 0;
 }
 

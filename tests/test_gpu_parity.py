@@ -227,9 +227,9 @@ def test_every_lane_group_size_against_oracle(group):
     np.testing.assert_allclose(_np(ep), epr, atol=1e-6)
 
 
-@pytest.mark.parametrize("env", [{"BIK_USE_TMA": 0}, {"BIK_SOLVE_PRECISION": "f32", "BIK_K2_PATH": "dense"}, {"BIK_K2_PATH": "dense"},
-                                 {"BIK_K2_PATH": "dense", "BIK_K2_WARPS": 4}, {"BIK_K2_GROUP": 4}, {"BIK_K2_GROUP": 8},
-                                 {"BIK_SOLVE_PRECISION": "f32"}, {"BIK_K1_PRECISION": "f64"}, {"BIK_K1_PRECISION": "f64", "BIK_K2_PATH": "dense"}])
+@pytest.mark.parametrize("env", [{"BIK_USE_TMA": 0}, {"BIK_K2_PATH": "dense"}, {"BIK_K2_PATH": "dense", "BIK_K2_WARPS": 4},
+                                 {"BIK_K2_GROUP": 4}, {"BIK_K2_GROUP": 8}, {"BIK_K1_PRECISION": "f64"},
+                                 {"BIK_K1_PRECISION": "f64", "BIK_K2_PATH": "dense"}])
 def test_alternate_paths(env):
     wl, fm, spec, g, model, prob = _engine("g1", env=env)
     q = torch.tensor(g["q"], dtype=torch.float32, device="cuda:0")
@@ -271,10 +271,10 @@ def test_k2_paths_agree_on_a_ragged_batch(name, path):
     assert err < 1e-4
 
 
-@pytest.mark.parametrize("env", [{}, {"BIK_K2_SWEEPS": 0}, {"BIK_K2_SWEEPS": 6}, {"BIK_K2_RULE": 0}, {"BIK_K2_DYNAMIC": 0},
-                                 {"BIK_K2_SWEEPS": 0, "BIK_K2_DYNAMIC": 0, "BIK_K2_GROUP": 4}, {"BIK_K1_GROUP": 8}])
+@pytest.mark.parametrize("env", [{}, {"BIK_K2_SWEEPS": 6}, {"BIK_K2_DYNAMIC": 0}, {"BIK_K2_DYNAMIC": 0, "BIK_K2_GROUP": 4},
+                                 {"BIK_K1_GROUP": 8}])
 def test_small_group_solver_knobs_against_oracle(env):
-    """Elimination of the unbounded dofs, Gauss-Seidel guess, release rule and tile hand-out only change HOW the optimum of
+    """Elimination of the unbounded dofs, Gauss-Seidel sweeps and tile hand-out only change HOW the optimum of
     mink's QP (solve_ik.py:43-105) is reached: every setting must return the oracle's dq on a ragged G1 batch with active
     bounds, and repeated launches on one stream must keep working (the tile counter rewinds itself)."""
     wl, fm, spec, g, model, prob = _engine("g1", env=env)
