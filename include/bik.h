@@ -233,6 +233,19 @@ int bik_converge(const bik_problem* problem, int B, float* q, const bik_inputs* 
                  double damping, int max_iters, float pos_threshold, float ori_threshold,
                  int check_every, int32_t* iters, int32_t* status, void* stream);
 
+/* The examples' outer loop (examples/arm_aloha.py:140-169): for each frame t of a target sequence, the bik_converge loop.
+ * Each instance moves to its next frame as soon as it is done with the current one; for every instance b the results are
+ * those of bik_converge called on frames 0..lengths[b]-1 in turn.  fp32 device buffers, as bik_converge.
+ *   in->frame_targets [B][T][F][7], in->com_targets [B][T][C][3]; posture targets as for bik_converge, the same for every frame
+ *   lengths [B] frames per instance, each in 0..T (NULL: all T); q [B][nq] in: start, out: end of each instance's last frame
+ *   q_traj [B][T][nq], iters [B][T], status [B][T] (NULL allowed): per frame, as bik_converge returns them; rows past
+ *   lengths[b] untouched
+ *   passes: device int, number of passes the loop ran, max_b sum_t (iters[b][t] + 1) (NULL allowed)
+ * BIK_CONVERGE_GRAPH=0 runs the host-polled loop: the device counter is read back every `check_every` passes. */
+int bik_track(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths,
+              float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every,
+              float* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+
 /* ---- fp64 entry points --------------------------------------------------------------------------------------------
  * The reference is fp64 end to end (numpy; mink/solve_ik.py:13-22).  These mirror the fp32 entry points above with
  * double buffers (bik_inputs.f64 = 1): the fp64 instantiations of the kernels run, on the kinematic constants at full

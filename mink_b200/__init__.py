@@ -28,7 +28,7 @@ def __getattr__(name):
         "ComTask": "tasks", "RelativeFrameTask": "tasks",
         "Limit": "limits", "Constraint": "limits", "ConfigurationLimit": "limits", "VelocityLimit": "limits",
         "CollisionAvoidanceLimit": "limits",
-        "build_ik": "ik", "solve_ik": "ik", "converge_ik": "ik",
+        "build_ik": "ik", "solve_ik": "ik", "converge_ik": "ik", "track_ik": "ik",
     }
     if name in table:
         return getattr(importlib.import_module(f"{__name__}.{table[name]}"), name)

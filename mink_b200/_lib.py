@@ -13,7 +13,7 @@ _lib = None
 EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destroy", "bik_problem_create",
            "bik_problem_destroy", "bik_problem_dims", "bik_fk", "bik_frame_jacobian", "bik_fk_jac",
            "bik_qp_objective", "bik_limits_box", "bik_solve", "bik_solve_ex", "bik_integrate", "bik_check_limits", "bik_step",
-           "bik_step_host", "bik_workspace_bytes", "bik_problem_describe", "bik_converge",
+           "bik_step_host", "bik_workspace_bytes", "bik_problem_describe", "bik_converge", "bik_track",
            "bik_fk64", "bik_frame_jacobian64", "bik_fk_jac64", "bik_qp_objective64", "bik_limits_box64", "bik_solve64",
            "bik_integrate64", "bik_check_limits64", "bik_step64", "bik_measure_fma_peak"]
 
@@ -62,6 +62,7 @@ def load():
     lib.bik_workspace_bytes.argtypes = [vp, ci]
     lib.bik_workspace_bytes.restype = C.c_size_t
     lib.bik_converge.argtypes = [vp, ci, vp, C.POINTER(BikInputs), cf, cd, ci, cf, cf, ci, vp, vp, vp]
+    lib.bik_track.argtypes = [vp, ci, ci, vp, C.POINTER(BikInputs), vp, cf, cd, ci, cf, cf, ci, vp, vp, vp, vp, vp]
     lib.bik_problem_describe.argtypes = [vp, cd, C.c_char_p, C.c_size_t]
     # fp64 mirror (double buffers, bik_inputs.f64 = 1)
     lib.bik_fk64.argtypes = lib.bik_fk.argtypes

@@ -75,6 +75,20 @@ __global__ void converge_finish_kernel(int B, int max_iters, const int32_t* __re
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b < B && !done[b]) { iters[b] = max_iters; if (status) status[b] |= 16; }
 }
+// bik_track bookkeeping: count = { passes run, instances with frames left, go }.  Every instance starts at frame 0, step 0
+// (step -1: no frames at all).  The tick counts a pass only when the previous one left work (so that the extra passes of the
+// host-polled loop are not counted) and rewinds the count that K1's test rebuilds; `go` = somebody still has frames left.
+__global__ void track_init_kernel(int B, int T, const int32_t* __restrict__ lengths, int32_t* cursor, int32_t* step, int* count) {
+  int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) { cursor[b] = 0; step[b] = (lengths ? lengths[b] : T) > 0 ? 0 : -1; }
+  if (b == 0) { count[0] = 0; count[1] = 0; count[2] = 1; }
+}
+__global__ void track_tick_kernel(int* count) { count[0] += count[2]; count[1] = 0; }
+__global__ void track_cond_kernel(int* count, cudaGraphConditionalHandle handle, int use_handle) {
+  const int go = count[1] > 0;
+  count[2] = go;
+  if (use_handle) cudaGraphSetConditional(handle, go ? 1u : 0u);
+}
 
 // CUDA-core FMA peak, measured: 16 independent dependent-chains of fused multiply-adds per thread, enough CTAs to fill every SM.
 // This is the denominator of K2's roofline (bench.py): the QP solve runs on the FMA pipes, not on tensor cores.
@@ -252,7 +266,7 @@ extern "C" void bik_problem_destroy(bik_problem* p) {
   conv_graph_drop(p);
   cudaFree(p->d_sched); cudaFree(p->d_image); cudaFree(p->pk); cudaFree(p->Gc); cudaFree(p->hc); cudaFree(p->warm);
   cudaFree(p->hq); cudaFree(p->hft); cudaFree(p->hpt); cudaFree(p->hct); cudaFree(p->hdq); cudaFree(p->hst);
-  cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_count);
+  cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_count); cudaFree(p->conv_cursor); cudaFree(p->conv_step); cudaFree(p->conv_status);
   if (p->conv_host) cudaFreeHost(p->conv_host);
   for (int i = 0; i < 4; ++i) if (p->hs[i]) cudaStreamDestroy(p->hs[i]);
   for (cudaEvent_t e : p->hev) cudaEventDestroy(e);
@@ -578,27 +592,41 @@ extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* 
 // sets (cudaGraphSetConditional), so the host enqueues one graph launch and never polls.  The graph is kept and reused as long
 // as the call's arguments do not change (the usual control loop).  BIK_CONVERGE_GRAPH=0, or any failure to build the graph,
 // falls back to a host loop that reads the device counter back every `check_every` steps.
+// bik_track (below) runs the same passes with K1 in track mode; `track` selects the mode everywhere in this driver.
+struct ConvCall {
+  int B, T, max_iters; float dt, pos, ori; double damping; float* q; const bik_inputs* in; const int32_t* lengths;
+  float* q_traj; int32_t *iters, *status; bool track, k1d;
+};
 struct ConvKey {
   int B, max_iters, check_every; float dt, pos, ori; double damping; const void *q, *ft, *pt, *ct, *iters, *status; int pb; bool k1d;
+  int track, T; const void *lengths, *q_traj;
   bool operator==(const ConvKey& o) const { return memcmp(this, &o, sizeof *this) == 0; }
 };
-static int converge_pass(bik_problem* p, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
-                         float ori_threshold, int32_t* iters, int32_t* status, bool k1d, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
-  converge_tick_kernel<<<1, 1, 0, st>>>(p->conv_count);
+// `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
+static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
+  const bik_inputs* in = c.in;
+  if (c.track) track_tick_kernel<<<1, 1, 0, st>>>(p->conv_count);
+  else converge_tick_kernel<<<1, 1, 0, st>>>(p->conv_count);
   K1Args a1;
   memset(&a1, 0, sizeof a1);
-  a1.B = B; a1.q = q; a1.ftgt = in->frame_targets; a1.ptgt = in->posture_targets; a1.ctgt = in->com_targets; a1.pbatched = in->posture_batched;
-  a1.dt = dt; a1.pk = p->pk; a1.Gc = p->Gc; a1.hc = p->hc;
-  a1.status = status; a1.tol = 1e-6f;
-  a1.done = p->conv_done; a1.iters = iters; a1.not_done = p->conv_count + 1; a1.conv_it = p->conv_count; a1.conv_max = max_iters;
-  a1.pos_thr = pos_threshold; a1.ori_thr = ori_threshold;
-  int rc = bik_launch_k1(p, a1, k1d, st);
+  a1.B = c.B; a1.q = c.q; a1.ftgt = in->frame_targets; a1.ptgt = in->posture_targets; a1.ctgt = in->com_targets; a1.pbatched = in->posture_batched;
+  a1.dt = c.dt; a1.pk = p->pk; a1.Gc = p->Gc; a1.hc = p->hc;
+  a1.status = c.track ? p->conv_status : status; a1.tol = 1e-6f;
+  a1.done = p->conv_done; a1.iters = c.iters; a1.not_done = p->conv_count + 1; a1.conv_it = p->conv_count; a1.conv_max = c.max_iters;
+  a1.pos_thr = c.pos; a1.ori_thr = c.ori;
+  if (c.track) {
+    a1.cursor = p->conv_cursor; a1.tstep = p->conv_step; a1.lengths = c.lengths; a1.T = c.T;
+    a1.q_traj = c.q_traj; a1.traj_status = status; a1.warm = p->warm;
+  }
+  int rc = bik_launch_k1(p, a1, c.k1d, st);
   if (rc) return rc;
-  converge_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, max_iters, handle, use_handle);
+  if (c.track) track_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, handle, use_handle);
+  else converge_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, c.max_iters, handle, use_handle);
   K2Args a2;
   memset(&a2, 0, sizeof a2);
-  a2.B = B; a2.q = q; a2.pk = p->pk; a2.pk64 = k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
-  a2.Gc = p->Gc; a2.hc = p->hc; a2.gc64 = k1d; a2.dt = dt; a2.damping = damping; a2.dq = p->conv_dq; a2.integrate = 1; a2.status = status;
+  a2.B = c.B; a2.q = c.q; a2.pk = p->pk; a2.pk64 = c.k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
+  a2.Gc = p->Gc; a2.hc = p->hc; a2.gc64 = c.k1d; a2.dt = c.dt; a2.damping = c.damping; a2.dq = p->conv_dq; a2.integrate = 1;
+  a2.status = c.track ? p->conv_status : status;
   a2.warm = p->warm; a2.skip = p->conv_done; a2.gate = p->conv_count + 2;
   rc = dispatch_k2(p, a2, st);
   if (rc) return rc;
@@ -623,29 +651,25 @@ static void conv_graph_drop(bik_problem* p) {
     }
 }
 
-extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
-                            float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, 0);
-  if (rc) return rc;
-  if (!q || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
-  if (check_every < 1) check_every = 1;
-  bik_problem* p = const_cast<bik_problem*>(cp);
+// The loop of bik_converge / bik_track.  Caller has validated the arguments.
+static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int32_t* passes, cudaStream_t st) {
   std::lock_guard<std::mutex> lock(p->mu);
   DeviceGuard g(p->model->device);
-  const bool k1d = k1_double(p, damping, false);
-  rc = ensure_workspace(p, B, k1d ? 8 : 4);
+  const int B = c.B;
+  int rc = ensure_workspace(p, B, c.k1d ? 8 : 4);
   if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const PHeader& h = p->h;
   rc = ws_acquire(p, st);
   if (rc) return rc;
   if ((size_t)B > p->conv_B) {
     conv_graph_drop(p);   // the cached graph captured the old buffers
-    cudaFree(p->conv_done); cudaFree(p->conv_dq);
-    p->conv_done = nullptr; p->conv_dq = nullptr; p->conv_B = 0;
+    cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_cursor); cudaFree(p->conv_step); cudaFree(p->conv_status);
+    p->conv_done = p->conv_cursor = p->conv_step = p->conv_status = nullptr; p->conv_dq = nullptr; p->conv_B = 0;
     CUDA_OK(cudaMalloc(&p->conv_done, sizeof(int32_t) * (size_t)B));
     CUDA_OK(cudaMalloc(&p->conv_dq, sizeof(float) * (size_t)B * h.nv));
+    CUDA_OK(cudaMalloc(&p->conv_cursor, sizeof(int32_t) * (size_t)B));
+    CUDA_OK(cudaMalloc(&p->conv_step, sizeof(int32_t) * (size_t)B));
+    CUDA_OK(cudaMalloc(&p->conv_status, sizeof(int32_t) * (size_t)B));
     p->conv_B = (size_t)B;
   }
   if (!p->conv_count) CUDA_OK(cudaMalloc(&p->conv_count, 4 * sizeof(int)));
@@ -656,9 +680,10 @@ extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_in
   if (graph_ok) {
     ConvKey key;
     memset(&key, 0, sizeof key);
-    key.B = B; key.max_iters = max_iters; key.check_every = 0; key.dt = dt; key.pos = pos_threshold; key.ori = ori_threshold; key.damping = damping;
-    key.q = q; key.ft = in->frame_targets; key.pt = in->posture_targets; key.ct = in->com_targets; key.iters = iters; key.status = status;
-    key.pb = in->posture_batched; key.k1d = k1d;
+    key.B = B; key.max_iters = c.max_iters; key.check_every = 0; key.dt = c.dt; key.pos = c.pos; key.ori = c.ori; key.damping = c.damping;
+    key.q = c.q; key.ft = c.in->frame_targets; key.pt = c.in->posture_targets; key.ct = c.in->com_targets; key.iters = c.iters; key.status = c.status;
+    key.pb = c.in->posture_batched; key.k1d = c.k1d;
+    key.track = c.track; key.T = c.T; key.lengths = c.lengths; key.q_traj = c.q_traj;
     {
       std::lock_guard<std::mutex> l2(g_conv_mu);
       for (auto& e : g_conv) if (e.first == p) cg = e.second;
@@ -666,16 +691,19 @@ extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_in
     if (cg && !(cg->key == key)) { conv_graph_drop(p); cg = nullptr; }
     if (!cg) {
       // warm the launch-geometry cache and the tile counter outside the capture (those paths allocate / query attributes):
-      // one K1 + a K2 that skips every instance
+      // one K1 + a K2 that skips every instance (track mode: every instance is marked as having no frames left).  The warm-up
+      // rewrites the loop state on its own stream, so an earlier call that may still be running on `st` finishes first.
+      CUDA_OK(cudaStreamSynchronize(st));
       bik_conv_graph ng;
       ng.key = key;
       bool built = false;
       do {
         if (cudaStreamCreateWithFlags(&ng.cap, cudaStreamNonBlocking) != cudaSuccess) break;
         cudaMemsetAsync(p->conv_done, 1, sizeof(int32_t) * (size_t)B, ng.cap);
+        if (c.track) cudaMemsetAsync(p->conv_step, 0xff, sizeof(int32_t) * (size_t)B, ng.cap);
         cudaMemsetAsync(p->conv_count, 0, 4 * sizeof(int), ng.cap);
         cudaGraphConditionalHandle none{};
-        if (converge_pass(p, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, iters, nullptr, k1d, none, 0, ng.cap) != BIK_OK) break;
+        if (converge_pass(p, c, nullptr, none, 0, ng.cap) != BIK_OK) break;
         if (cudaStreamSynchronize(ng.cap) != cudaSuccess) break;
         if (cudaGraphCreate(&ng.graph, 0) != cudaSuccess) break;
         cudaGraphConditionalHandle handle;
@@ -686,7 +714,7 @@ extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_in
         if (cudaGraphAddNode(&node, ng.graph, nullptr, 0, &cp2) != cudaSuccess) break;
         cudaGraph_t body = cp2.conditional.phGraph_out[0];
         if (cudaStreamBeginCaptureToGraph(ng.cap, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess) break;
-        const int prc = converge_pass(p, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, iters, status, k1d, handle, 1, ng.cap);
+        const int prc = converge_pass(p, c, c.status, handle, 1, ng.cap);
         if (cudaStreamEndCapture(ng.cap, nullptr) != cudaSuccess || prc != BIK_OK) break;
         if (cudaGraphInstantiate(&ng.exec, ng.graph, 0) != cudaSuccess) break;
         built = true;
@@ -704,28 +732,85 @@ extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_in
       }
     }
   }
-  CUDA_OK(cudaMemsetAsync(p->conv_done, 0, sizeof(int32_t) * (size_t)B, st));
-  CUDA_OK(cudaMemsetAsync(p->conv_count, 0xff, sizeof(int), st));   // step counter = -1: the first tick makes it 0
+  if (c.track) {
+    track_init_kernel<<<blocks, 128, 0, st>>>(B, c.T, c.lengths, p->conv_cursor, p->conv_step, p->conv_count);
+    CUDA_OK(cudaGetLastError());
+  } else {
+    CUDA_OK(cudaMemsetAsync(p->conv_done, 0, sizeof(int32_t) * (size_t)B, st));
+    CUDA_OK(cudaMemsetAsync(p->conv_count, 0xff, sizeof(int), st));   // step counter = -1: the first tick makes it 0
+  }
   CUDA_OK(cudaMemsetAsync(p->warm, 0, (size_t)B * (size_t)(h.nu > 0 ? h.nu : 1), st));
   if (graph_ok && cg) {
     CUDA_OK(cudaGraphLaunch(cg->exec, st));
   } else {
+    // converge: passes 0..max_iters, polled after step `it` every check_every steps; track: at most T frames of max_iters + 1
+    // passes each, polled every check_every passes
+    const long long cap = c.track ? (long long)c.T * (c.max_iters + 1) : (long long)c.max_iters + 1;
     bool all_done = false;
     cudaGraphConditionalHandle none{};
-    for (int it = 0; it <= max_iters && !all_done; ++it) {
-      rc = converge_pass(p, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, iters, status, k1d, none, 0, st);
+    for (long long it = 0; it < cap && !all_done; ++it) {
+      rc = converge_pass(p, c, c.status, none, 0, st);
       if (rc) return rc;
-      if (it > 0 && (it == max_iters || it % check_every == 0)) {   // errors at the configuration reached after `it` steps
+      const bool poll = c.track ? ((it + 1) % check_every == 0 || it + 1 == cap) : (it > 0 && (it == c.max_iters || it % check_every == 0));
+      if (poll) {
         CUDA_OK(cudaMemcpyAsync(p->conv_host, p->conv_count, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
         CUDA_OK(cudaStreamSynchronize(st));
         all_done = p->conv_host[1] == 0;
       }
     }
   }
-  // instances that never met the thresholds: iters = max_iters, status bit BIK_STATUS_NOT_CONVERGED
-  converge_finish_kernel<<<blocks, 128, 0, st>>>(B, max_iters, p->conv_done, iters, status);
-  CUDA_OK(cudaGetLastError());
+  if (c.track) {
+    if (passes) CUDA_OK(cudaMemcpyAsync(passes, p->conv_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  } else {
+    // instances that never met the thresholds: iters = max_iters, status bit BIK_STATUS_NOT_CONVERGED
+    converge_finish_kernel<<<blocks, 128, 0, st>>>(B, c.max_iters, p->conv_done, c.iters, c.status);
+    CUDA_OK(cudaGetLastError());
+  }
   return ws_release(p, st, BIK_OK);
+}
+
+extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
+                            float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+  if (B == 0 && cp) return BIK_OK;
+  int rc = check_inputs(cp, in, false, 0);
+  if (rc) return rc;
+  if (!q || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
+  if (check_every < 1) check_every = 1;
+  bik_problem* p = const_cast<bik_problem*>(cp);
+  ConvCall c;
+  memset(&c, 0, sizeof c);
+  c.B = B; c.T = 1; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
+  c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, false);
+  return converge_run(p, c, check_every, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+// The examples' outer loop: for each frame of a target sequence, the bik_converge loop, every instance on its own cursor.
+// One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
+// moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
+extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
+                         int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
+                         int32_t* passes, void* stream) {
+  if (B == 0 && cp) return BIK_OK;
+  int rc = check_inputs(cp, in, false, 0);
+  if (rc) return rc;
+  if (!q || !q_traj || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
+  if (T < 1) return bik_fail(BIK_ERR_INVALID, "T must be at least 1");
+  if (check_every < 1) check_every = 1;
+  bik_problem* p = const_cast<bik_problem*>(cp);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (lengths) {   // a length beyond T would read another instance's targets: check them before anything is enqueued
+    DeviceGuard g(p->model->device);
+    std::vector<int32_t> hl((size_t)B);
+    CUDA_OK(cudaMemcpyAsync(hl.data(), lengths, sizeof(int32_t) * (size_t)B, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    for (int b = 0; b < B; ++b)
+      if (hl[b] < 0 || hl[b] > T) return bik_fail(BIK_ERR_INVALID, "lengths[" + std::to_string(b) + "] = " + std::to_string(hl[b]) + " is outside 0..T");
+  }
+  ConvCall c;
+  memset(&c, 0, sizeof c);
+  c.B = B; c.T = T; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
+  c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = true; c.k1d = k1_double(p, damping, false);
+  return converge_run(p, c, check_every, passes, st);
 }
 
 // Host-buffer variant: device staging lives in the problem (separate allocations).  The batch is cut into chunks that flow

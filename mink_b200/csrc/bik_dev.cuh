@@ -107,6 +107,10 @@ struct bik_problem {
   float* conv_dq = nullptr;
   int* conv_count = nullptr;   // device: { steps taken so far, unconverged instances }
   int* conv_host = nullptr;    // pinned mirror
+  // bik_track state (the same loop, per-instance frame cursor)
+  int32_t* conv_cursor = nullptr;   // [B] frame each instance is on
+  int32_t* conv_step = nullptr;     // [B] steps taken in that frame, -1 = no frames left
+  int32_t* conv_status = nullptr;   // [B] status of the frame in progress
 };
 
 // resident CTAs per SM for (kernel, dynamic smem, threads): attribute + occupancy queries run once per combination

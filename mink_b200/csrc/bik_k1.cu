@@ -10,7 +10,7 @@ using namespace bik;
                              // H100 (700 W), G1 at 65 536: K1 of the step 0.090 ms, dense API form 0.213 ms; 5 -> 96 registers with
                              // 44-64 B of spill stores: 0.094 / 0.286 ms
 #endif
-template <typename T, int G, bool PK>
+template <typename T, int G, bool PK, bool TR>
 __global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K1Args a) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ __align__(8) uint64_t bar;
@@ -33,15 +33,15 @@ __global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1
       asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncwarp();
-    if (tile < ntiles && k1_tile_bulk_ok<T>(h, a, tile * IPW, IPW)) {
+    if (tile < ntiles && k1_tile_bulk_ok<T, TR>(h, a, tile * IPW, IPW)) {
       T* qtile = wsm + k1_qtile_offset(h, IPW);
-      if (lane == 0) k1_pipe_arm<T>(h, a, tile * IPW, IPW, &pipe, qtile, qtile + ((IPW * h.nq + 3) & ~3));
+      if (lane == 0) k1_pipe_arm<T, TR>(h, a, tile * IPW, IPW, &pipe, qtile, qtile + ((IPW * h.nq + 3) & ~3));
       pipe.armed = tile * IPW;
     }
   }
   for (; tile < ntiles; tile += stride) {
     const int next = tile + stride < ntiles ? (tile + stride) * IPW : -1;
-    k1_warp_tile<T, G, 32, PK>(P, a, tile * IPW, wsm, lane, pp, next);
+    k1_warp_tile<T, G, 32, PK, TR>(P, a, tile * IPW, wsm, lane, pp, next);
   }
 }
 
@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(128) fk_kernel(const uint32_t* __restrict__ gi
   for (int tile = blockIdx.x * nwarps + warp; tile < ntiles; tile += gridDim.x * nwarps) fk_warp_tile<T, G, 32>(P, a, tile * IPW, wsm, lane);
 }
 
-template <typename T, int G, bool PK>
+template <typename T, int G, bool PK, bool TR>
 static int launch_k1_pk(const bik_problem* p, const K1Args& a, cudaStream_t st) {
   const PHeader& h = p->h;
   constexpr int IPW = 32 / G;
@@ -69,15 +69,16 @@ static int launch_k1_pk(const bik_problem* p, const K1Args& a, cudaStream_t st) 
   size_t smem = need(NW);
   int grid = 1;
   long long tiles = ((long long)a.B + IPW - 1) / IPW;
-  int rc = bik_launch_geometry((const void*)k1_kernel<T, G, PK>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
+  int rc = bik_launch_geometry((const void*)k1_kernel<T, G, PK, TR>, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
   if (rc) return rc;
-  k1_kernel<T, G, PK><<<grid, 32 * NW, smem, st>>>(p->d_image, words, p->model->use_tma, a);
+  k1_kernel<T, G, PK, TR><<<grid, 32 * NW, smem, st>>>(p->d_image, words, p->model->use_tma, a);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
 template <typename T, int G>
 static int launch_k1(const bik_problem* p, const K1Args& a, cudaStream_t st) {
-  return a.pk ? launch_k1_pk<T, G, true>(p, a, st) : launch_k1_pk<T, G, false>(p, a, st);
+  if (!a.pk) return launch_k1_pk<T, G, false, false>(p, a, st);
+  return a.cursor ? launch_k1_pk<T, G, true, true>(p, a, st) : launch_k1_pk<T, G, true, false>(p, a, st);
 }
 template <typename T>
 static int dispatch_k1(const bik_problem* p, const K1Args& a, cudaStream_t st) {

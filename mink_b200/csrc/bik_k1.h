@@ -153,6 +153,18 @@ struct K1Args {
   const int* conv_it;    // device counter: steps taken so far (0: nothing is tested yet)
   int conv_max;          // max_iters: at step conv_max nothing is solved any more, so the limits are not checked either
   float pos_thr, ori_thr;
+  // track mode of bik_track (the TR instantiation): the same test, but every instance walks its own sequence of frames.
+  // The step index is per instance; a test that ends a frame writes iters / traj_status / q_traj at row b*T + cursor[b],
+  // clears b's warm-start bytes and moves the cursor on.  done[] is rewritten on every pass: 1 = K2 leaves b alone in this
+  // pass (its frame just ended, or it has no frames left); *not_done counts the instances with frames left; status is
+  // the [B] status of the frame in progress.  iters is [B][T] here.
+  int32_t* cursor;       // [B] frame each instance is on
+  int32_t* tstep;        // [B] steps taken in that frame; -1: no frames left (nothing is computed for the instance)
+  const int32_t* lengths;   // [B] frames per instance, or null: all T
+  int T;
+  float* q_traj;         // [B][T][nq]
+  int32_t* traj_status;  // [B][T] or null
+  signed char* warm;     // [B][max(nu,1)] K2's warm-start bytes
 };
 
 // ---- per-warp scratch layout (elements of T) --------------------------------------------------
@@ -189,7 +201,8 @@ struct K1Pipe {
   int armed;
 };
 // Bulk copies need 16-byte sizes and addresses, and the buffers must hold the kernel's scalar type (fp32 kernel, fp32 inputs).
-template <typename T>
+// TR (track mode): only the q rows travel this way; a tile's targets are rows of different frames, loaded per instance.
+template <typename T, bool TR = false>
 BIK_HD bool k1_tile_bulk_ok(const PHeader& h, const K1Args& a, int inst0, int ipw) {
   if (sizeof(T) != 4 || a.in64 || inst0 < 0 || inst0 >= a.B) return false;
   const int nvalid = (a.B - inst0) < ipw ? (a.B - inst0) : ipw;
@@ -197,16 +210,17 @@ BIK_HD bool k1_tile_bulk_ok(const PHeader& h, const K1Args& a, int inst0, int ip
   const size_t qa = reinterpret_cast<size_t>(a.q) + (size_t)inst0 * h.nq * 4, fa = reinterpret_cast<size_t>(a.ftgt) + (size_t)inst0 * h.F * 7 * 4,
                ca = reinterpret_cast<size_t>(a.ctgt) + (size_t)inst0 * h.C * 3 * 4;
   if ((qb | qa) & 15) return false;
+  if (TR) return true;
   if (h.F > 0 && ((fb | fa | ((size_t)ipw * h.F * 7 * 4)) & 15)) return false;   // (the CoM targets sit behind a full tile of frame targets)
   if (h.C > 0 && ((cb | ca) & 15)) return false;
   return true;
 }
 #if defined(__CUDACC__)
 // lane 0 of the warp: arm the barrier with the byte count and issue the copies of the tile starting at inst0
-template <typename T>
+template <typename T, bool TR = false>
 __device__ __forceinline__ void k1_pipe_arm(const PHeader& h, const K1Args& a, int inst0, int ipw, K1Pipe* pipe, T* qtile, T* ttile) {
   const int nvalid = (a.B - inst0) < ipw ? (a.B - inst0) : ipw;
-  const uint32_t qb = (uint32_t)nvalid * h.nq * 4, fb = (uint32_t)nvalid * h.F * 7 * 4, cb = (uint32_t)nvalid * h.C * 3 * 4;
+  const uint32_t qb = (uint32_t)nvalid * h.nq * 4, fb = TR ? 0u : (uint32_t)nvalid * h.F * 7 * 4, cb = TR ? 0u : (uint32_t)nvalid * h.C * 3 * 4;
   mbar_expect_tx(pipe->bar, qb + fb + cb);
   bulk_g2s(qtile, reinterpret_cast<const float*>(a.q) + (size_t)inst0 * h.nq, qb, pipe->bar);
   if (fb) bulk_g2s(ttile, reinterpret_cast<const float*>(a.ftgt) + (size_t)inst0 * h.F * 7, fb, pipe->bar);
@@ -511,15 +525,17 @@ template <> BIK_HD void store6<double>(double* o, V3<double> top, V3<double> bot
 // One warp tile: instances [inst0, inst0 + IPW) clipped to B.
 // PK (compile time): packed hand-off with the fused check_limits / convergence test (bik_step, bik_converge), else the dense
 // API form (bik_fk_jac) -- two instantiations so that neither carries the other's registers and code.
-template <typename T, int G, int W, bool PK>
+// TR (compile time, with PK): track mode of bik_track (see K1Args); a third instantiation, so the other two are unchanged.
+template <typename T, int G, int W, bool PK, bool TR = false>
 BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int lane, K1Pipe* pipe = nullptr, int next_inst0 = -1) {
+  static_assert(!TR || PK, "track mode writes the packed hand-off");
   const PHeader& h = P.h();
   constexpr int IPW = W / G;
   const int nv = h.nv, nq = h.nq, K = h.K;
   const int li = lane / G, g = lane % G;
   const int b = inst0 + li;
   const int nvalid = (a.B - inst0) < IPW ? (a.B - inst0) : IPW;
-  const bool valid = li < nvalid;
+  const bool valid = li < nvalid && (!TR || a.tstep[b] >= 0);   // track mode: an instance without frames left does no work
   const int SS = k1_state_stride(h);
   constexpr bool packed = PK;
   const long long PKS = h.pk_stride;
@@ -548,8 +564,19 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
     if (!landed) {
       const long long q0 = (long long)inst0 * nq, f0 = (long long)inst0 * h.F * 7, c0 = (long long)inst0 * h.C * 3;
       for (int k = lane; k < nvalid * nq; k += W) qtile[k] = ldin<T>(a.q, q0 + k, a.in64);
-      for (int k = lane; k < nvalid * h.F * 7; k += W) ttile[k] = ldin<T>(a.ftgt, f0 + k, a.in64);
-      for (int k = lane; k < nvalid * h.C * 3; k += W) ttile[IPW * h.F * 7 + k] = ldin<T>(a.ctgt, c0 + k, a.in64);
+      if (!TR) {
+        for (int k = lane; k < nvalid * h.F * 7; k += W) ttile[k] = ldin<T>(a.ftgt, f0 + k, a.in64);
+        for (int k = lane; k < nvalid * h.C * 3; k += W) ttile[IPW * h.F * 7 + k] = ldin<T>(a.ctgt, c0 + k, a.in64);
+      }
+    }
+    if (TR) {   // the targets of each instance's current frame: row b*T + cursor[b] of the [B][T] sequences
+      const int FW = h.F * 7, CW = h.C * 3;
+      for (int i = 0; i < nvalid; ++i) {
+        if (a.tstep[inst0 + i] < 0) continue;
+        const long long row = (long long)(inst0 + i) * a.T + a.cursor[inst0 + i];
+        for (int k = lane; k < FW; k += W) ttile[i * FW + k] = ldin<T>(a.ftgt, row * FW + k, a.in64);
+        for (int k = lane; k < CW; k += W) ttile[IPW * FW + i * CW + k] = ldin<T>(a.ctgt, row * CW + k, a.in64);
+      }
     }
     if (PK && a.status && lane < IPW) sflag[lane] = 0;
   }
@@ -558,13 +585,15 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
 
   // ---- Configuration.check_limits (configuration.py:77-110), fused: every lane tests a few dofs of the tile ----
   // inside bik_converge the step index lives on the device (the loop may be a CUDA-graph WHILE node: no host in between)
-  const int conv_step = (PK && a.done) ? *a.conv_it : 0;
-  const bool do_check = PK && a.status && !(a.done && conv_step >= a.conv_max);
+  // (track mode: the same rules with each instance's own step index)
+  const int conv_step = (PK && !TR && a.done) ? *a.conv_it : 0;
+  const bool do_check = PK && a.status && !(!TR && a.done && conv_step >= a.conv_max);
   const bool accumulate = a.done ? conv_step > 0 : a.accumulate != 0;
   if (do_check) {
     const int32_t* dofqadr = P.i(h.off_dofqadr);
     const float* rng = P.f(h.off_range);
     for (int i = 0; i < nvalid; ++i) {
+      if (TR) { const int s = a.tstep[inst0 + i]; if (s < 0 || s >= a.conv_max) continue; }
       int bad = 0;
       for (int d = lane; d < nv; d += W) {
         const int qa = dofqadr[d];
@@ -582,7 +611,12 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
       }
     }
     BIK_SYNCWARP();
-    if (lane < nvalid) a.status[inst0 + lane] = accumulate ? (a.status[inst0 + lane] | sflag[lane]) : sflag[lane];
+    if (TR) {
+      const int s = lane < nvalid ? a.tstep[inst0 + lane] : -1;
+      if (s >= 0 && s < a.conv_max) a.status[inst0 + lane] = s > 0 ? (a.status[inst0 + lane] | sflag[lane]) : sflag[lane];
+    } else if (lane < nvalid) {
+      a.status[inst0 + lane] = accumulate ? (a.status[inst0 + lane] | sflag[lane]) : sflag[lane];
+    }
   }
 
   // ---- forward kinematics over the lane program --------------------------------------------
@@ -655,8 +689,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
   BIK_SYNCWARP();
   // ---- the tile's inputs are dead from here on: send the next tile's ahead (bulk async copies into the same buffers) ----
 #if defined(__CUDA_ARCH__)
-  if (pipe && k1_tile_bulk_ok<T>(h, a, next_inst0, IPW)) {
-    if (lane == 0) k1_pipe_arm<T>(h, a, next_inst0, IPW, pipe, qtile, ttile);
+  if (pipe && k1_tile_bulk_ok<T, TR>(h, a, next_inst0, IPW)) {
+    if (lane == 0) k1_pipe_arm<T, TR>(h, a, next_inst0, IPW, pipe, qtile, ttile);
     pipe->armed = next_inst0;
   }
 #endif
@@ -776,7 +810,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
   }
 
   // ---- convergence test of the examples' inner loop (bik_converge), on the unweighted frame errors --------
-  if (PK && a.done) {
+  if (PK && !TR && a.done) {
     BIK_SYNCWARP();
     const int it = conv_step;
     if (it > 0 && lane < nvalid && !a.done[inst0 + lane]) {
@@ -795,6 +829,60 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
 #endif
       }
     }
+  }
+  // ---- track mode (bik_track): the same test ends the instance's frame instead of the call -----------------------------
+  // A frame ends when its errors pass after at least one step, or after max_iters steps (then with BIK_STATUS_NOT_CONVERGED);
+  // its results are those of a bik_converge call on that frame.  The next pass starts the next frame at step 0 with a cold
+  // warm start, exactly as a new bik_converge call does.
+  if (TR) {
+    BIK_SYNCWARP();
+    int ended = -1;   // frame of instance inst0 + lane that ends in this pass
+    if (lane < nvalid) {
+      const int bi = inst0 + lane, s = a.tstep[bi];
+      int skip = 1, left = 0;
+      if (s >= 0) {
+        bool ok = s > 0;
+        for (int f = 0; ok && f < h.F; ++f) {
+          const T* eb = estage + lane * K + P.frame(f).row0;
+          const T pos = bik_sqrt<T>(eb[0] * eb[0] + eb[1] * eb[1] + eb[2] * eb[2]), ori = bik_sqrt<T>(eb[3] * eb[3] + eb[4] * eb[4] + eb[5] * eb[5]);
+          ok = pos <= T(a.pos_thr) && ori <= T(a.ori_thr);
+        }
+        if (ok || s >= a.conv_max) {
+          const int c = a.cursor[bi];
+          const long long row = (long long)bi * a.T + c;
+          a.iters[row] = s;
+          if (a.traj_status) a.traj_status[row] = a.status[bi] | (ok ? 0 : 16);
+          ended = c;
+          left = c + 1 < (a.lengths ? a.lengths[bi] : a.T);
+          a.cursor[bi] = c + 1;
+          a.tstep[bi] = left ? 0 : -1;
+        } else {
+          a.tstep[bi] = s + 1;
+          skip = 0; left = 1;
+        }
+      }
+      a.done[bi] = skip;
+      if (left) {
+#if defined(__CUDA_ARCH__)
+        atomicAdd(a.not_done, 1);
+#else
+        *a.not_done += 1;
+#endif
+      }
+    }
+    if (lane < IPW) sflag[lane] = ended;
+    BIK_SYNCWARP();
+    // q_traj rows of the frames that ended (from global q: the tile's copy may already hold the next tile's rows), and a cold
+    // warm start for the next frame
+    const float* qg = reinterpret_cast<const float*>(a.q);
+    for (int k = lane; k < nvalid * nq; k += W) {
+      const int i = k / nq, c = sflag[i];
+      if (c >= 0) a.q_traj[((long long)(inst0 + i) * a.T + c) * nq + (k - i * nq)] = qg[(long long)inst0 * nq + k];
+    }
+    const int nw = h.nu > 0 ? h.nu : 1;
+    for (int k = lane; k < nvalid * nw; k += W)
+      if (sflag[k / nw] >= 0) a.warm[(long long)inst0 * nw + k] = 0;
+    BIK_SYNCWARP();
   }
 
   // ---- task errors out (contiguous IPW x K run) ------------------------------------------------

@@ -14,6 +14,7 @@ import numpy as np
 
 from ._abi import ProblemSpec
 from .configuration import Configuration
+from .exceptions import InvalidTarget
 from .limits import ConfigurationLimit, Limit
 from .tasks import ComTask, FrameTask, PostureTask, Task, problem_for
 
@@ -27,27 +28,39 @@ class Problem(NamedTuple):
     h: Optional[object]
 
 
-def _lower(configuration: Configuration, tasks: Sequence[Task], limits: Optional[Sequence[Limit]]):
+def _problem(configuration: Configuration, tasks: Sequence[Task], limits: Optional[Sequence[Limit]]):
     flat = configuration.flat
     if limits is None:   # default of the reference (solve_ik.py:28-29)
         limits = [ConfigurationLimit(configuration.model)]
-    # libbik stacks rows by task kind order of appearance; keep frame / com targets in list order
     tspecs = [t._spec(flat) for t in tasks]
     lspecs = [s for s in (l._spec(flat) for l in limits) if s is not None]
-    spec = ProblemSpec(tspecs, lspecs)
+    return problem_for(configuration, ProblemSpec(tspecs, lspecs)), limits
+
+
+def _posture_targets(tasks: Sequence[Task], nq: int):
+    pt = [np.asarray(t._target()).reshape(-1, nq) for t in tasks if isinstance(t, PostureTask)]
+    if not pt:
+        return None
+    nb = max(p.shape[0] for p in pt)
+    return np.stack([np.broadcast_to(p, (nb, nq)) for p in pt], axis=1)
+
+
+def _lower(configuration: Configuration, tasks: Sequence[Task], limits: Optional[Sequence[Limit]]):
+    flat = configuration.flat
+    prob, limits = _problem(configuration, tasks, limits)
+    # libbik stacks rows by task kind order of appearance; keep frame / com targets in list order
     B = configuration.q_device.shape[0]
     ft = [np.broadcast_to(np.asarray(t._target()).reshape(-1, 7), (B, 7)) for t in tasks if isinstance(t, FrameTask)]
-    pt = [np.asarray(t._target()).reshape(-1, flat.nq) for t in tasks if isinstance(t, PostureTask)]
+    pt = _posture_targets(tasks, flat.nq)
     ct = [np.broadcast_to(np.asarray(t._target()).reshape(-1, 3), (B, 3)) for t in tasks if isinstance(t, ComTask)]
     kw = {}
     if ft:
         kw["frame_targets"] = np.stack(ft, axis=1)
-    if pt:
-        nb = max(p.shape[0] for p in pt)
-        kw["posture_targets"] = np.stack([np.broadcast_to(p, (nb, flat.nq)) for p in pt], axis=1)
+    if pt is not None:
+        kw["posture_targets"] = pt
     if ct:
         kw["com_targets"] = np.stack(ct, axis=1)
-    return problem_for(configuration, spec), kw, limits
+    return prob, kw, limits
 
 
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
@@ -123,3 +136,75 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     if configuration.batched:
         return it, ok
     return int(it[0]), bool(ok[0])
+
+
+def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
+             damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
+             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1):
+    """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
+
+        for t in range(T):
+            for task, seq in targets.items(): task.set_target(seq[t])
+            converge_ik(configuration, tasks, dt, solver, damping, limits, max_iters, pos_threshold, ori_threshold)
+
+    with every instance of a batch moving to its next frame as soon as it is done with the current one.
+
+    `targets` maps a FrameTask / RelativeFrameTask to its [T, 7] or [B, T, 7] sequence (an SE3 or an array / tensor,
+    wxyz_xyz) and a ComTask to its [T, 3] or [B, T, 3] sequence; a sequence without a batch dimension is shared by every
+    instance, and a task not in `targets` keeps its current target.  CUDA tensors are used where they are.  `lengths`
+    ([B], each in 0..T) ends instance b's sequence after lengths[b] frames.  The configuration ends at its final q.
+
+    Returns (q_traj, iters, converged) per frame: numpy [T, nq] / [T] / [T] for a single configuration, torch CUDA
+    [B, T, nq] / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
+    import torch
+
+    for task in targets:
+        if not isinstance(task, (FrameTask, ComTask)):
+            raise InvalidTarget(f"track_ik takes target sequences for FrameTask, RelativeFrameTask and ComTask, not {type(task).__name__}")
+    flat = configuration.flat
+    q = configuration.q_device
+    B, dev = q.shape[0], q.device
+    held = [t for t in tasks if isinstance(t, (FrameTask, ComTask)) and t not in targets]
+    for t in held:
+        t._target()   # TargetNotSet when a task has neither a sequence nor a target
+    seqs, T = {}, None
+    for task, seq in targets.items():
+        k = 7 if isinstance(task, FrameTask) else 3
+        if hasattr(seq, "wxyz_xyz"):
+            seq = seq.wxyz_xyz
+        s = seq if isinstance(seq, torch.Tensor) else torch.as_tensor(np.asarray(seq, dtype=np.float32))
+        s = s.to(device=dev, dtype=torch.float32)
+        if s.ndim == 2:
+            s = s.unsqueeze(0).expand(B, -1, -1)
+        if s.ndim != 3 or s.shape[0] != B or s.shape[2] != k or s.shape[1] < 1:
+            raise InvalidTarget(f"Expected a [T, {k}] or [{B}, T, {k}] target sequence for {type(task).__name__}, got {tuple(s.shape)}")
+        if T is not None and s.shape[1] != T:
+            raise InvalidTarget(f"target sequences of different lengths: {T} and {s.shape[1]} frames")
+        T = s.shape[1]
+        seqs[task] = s
+    if T is None:
+        raise InvalidTarget("track_ik needs at least one FrameTask / RelativeFrameTask / ComTask target sequence")
+
+    def stacked(kind, k):
+        rows = [seqs[t] if t in seqs else torch.as_tensor(np.asarray(t._target(), dtype=np.float32).reshape(-1, 1, k), device=dev).expand(B, T, k)
+                for t in tasks if isinstance(t, kind)]
+        return torch.stack(rows, dim=2).contiguous() if rows else None
+
+    prob, limits = _problem(configuration, tasks, limits)
+    ln = None
+    if lengths is not None:
+        ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
+        if ln.shape != (B,):
+            raise InvalidTarget(f"lengths must have shape ({B},), got {tuple(ln.shape)}")
+    q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), _posture_targets(tasks, flat.nq), stacked(ComTask, 3), lengths=ln, dt=dt,
+                                          damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
+                                          ori_threshold=ori_threshold, check_every=check_every)
+    configuration._sync_from_device()
+    ran = iters >= 0
+    bad = ((status & (2 | 4 | 8)) != 0) & ran
+    n_bad = int(bad.sum())
+    assert n_bad == 0, f"QP not solved for {n_bad} frame(s) (status bits {np.unique((status[bad] & 14).cpu().numpy())})"
+    converged = ran & ((status & 16) == 0)
+    if configuration.batched:
+        return q_traj, iters, converged
+    return q_traj[0].cpu().numpy().astype(np.float64), iters[0].cpu().numpy(), converged[0].cpu().numpy()
