@@ -235,7 +235,7 @@ int bik_converge(const bik_problem* problem, int B, float* q, const bik_inputs* 
 
 /* The examples' outer loop (examples/arm_aloha.py:140-169): for each frame t of a target sequence, the bik_converge loop.
  * Each instance moves to its next frame as soon as it is done with the current one; for every instance b the results are
- * those of bik_converge called on frames 0..lengths[b]-1 in turn.  fp32 device buffers, as bik_converge.
+ * those of bik_converge called on frames 0..lengths[b]-1 in turn.  fp32 device buffers, as bik_converge (bik_track64: fp64).
  *   in->frame_targets [B][T][F][7], in->com_targets [B][T][C][3]; posture targets as for bik_converge, the same for every frame
  *   lengths [B] frames per instance, each in 0..T (NULL: all T); q [B][nq] in: start, out: end of each instance's last frame
  *   q_traj [B][T][nq], iters [B][T], status [B][T] (NULL allowed): per frame, as bik_converge returns them; rows past
@@ -271,6 +271,15 @@ int bik_check_limits64(const bik_model* model, int B, const double* q, double to
                        void* stream);
 int bik_step64(const bik_problem* problem, int B, double* q, const bik_inputs* in, double dt,
                double damping, int nsteps, int integrate, double* dq, int32_t* status, void* stream);
+/* bik_converge and bik_track on fp64 buffers (q, q_traj and the targets are double; in->f64 = 1 is required): the same
+ * loops, the same arguments and results, with the fp64 K1 and the thresholds compared in double as the reference compares
+ * them.  The fp32 bik_converge / bik_track reject fp64 inputs, and these reject fp32 ones. */
+int bik_converge64(const bik_problem* problem, int B, double* q, const bik_inputs* in, double dt, double damping,
+                   int max_iters, double pos_threshold, double ori_threshold, int check_every,
+                   int32_t* iters, int32_t* status, void* stream);
+int bik_track64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths,
+                double dt, double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
+                double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
 
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */

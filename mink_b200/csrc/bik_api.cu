@@ -593,13 +593,15 @@ extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* 
 // as the call's arguments do not change (the usual control loop).  BIK_CONVERGE_GRAPH=0, or any failure to build the graph,
 // falls back to a host loop that reads the device counter back every `check_every` steps.
 // bik_track (below) runs the same passes with K1 in track mode; `track` selects the mode everywhere in this driver.
+// io64: fp64 buffers (bik_converge64 / bik_track64), the fp64 K1; dt and the thresholds of fp32 calls are their float values.
 struct ConvCall {
-  int B, T, max_iters; float dt, pos, ori; double damping; float* q; const bik_inputs* in; const int32_t* lengths;
-  float* q_traj; int32_t *iters, *status; bool track, k1d;
+  int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
+  void* q_traj; int32_t *iters, *status; bool track, k1d, io64;
 };
 struct ConvKey {
-  int B, max_iters, check_every; float dt, pos, ori; double damping; const void *q, *ft, *pt, *ct, *iters, *status; int pb; bool k1d;
+  int B, max_iters, check_every; double dt, pos, ori; double damping; const void *q, *ft, *pt, *ct, *iters, *status; int pb; bool k1d;
   int track, T; const void *lengths, *q_traj;
+  int io64;   // a buffer freed by one precision's caller may come back at the same address for the other's
   bool operator==(const ConvKey& o) const { return memcmp(this, &o, sizeof *this) == 0; }
 };
 // `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
@@ -610,10 +612,10 @@ static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cud
   K1Args a1;
   memset(&a1, 0, sizeof a1);
   a1.B = c.B; a1.q = c.q; a1.ftgt = in->frame_targets; a1.ptgt = in->posture_targets; a1.ctgt = in->com_targets; a1.pbatched = in->posture_batched;
-  a1.dt = c.dt; a1.pk = p->pk; a1.Gc = p->Gc; a1.hc = p->hc;
+  a1.in64 = c.io64; a1.dt = c.dt; a1.pk = p->pk; a1.Gc = p->Gc; a1.hc = p->hc;
   a1.status = c.track ? p->conv_status : status; a1.tol = 1e-6f;
   a1.done = p->conv_done; a1.iters = c.iters; a1.not_done = p->conv_count + 1; a1.conv_it = p->conv_count; a1.conv_max = c.max_iters;
-  a1.pos_thr = c.pos; a1.ori_thr = c.ori;
+  a1.pos_thr = (float)c.pos; a1.ori_thr = (float)c.ori; a1.pos_thr64 = c.pos; a1.ori_thr64 = c.ori;
   if (c.track) {
     a1.cursor = p->conv_cursor; a1.tstep = p->conv_step; a1.lengths = c.lengths; a1.T = c.T;
     a1.q_traj = c.q_traj; a1.traj_status = status; a1.warm = p->warm;
@@ -624,7 +626,7 @@ static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cud
   else converge_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, c.max_iters, handle, use_handle);
   K2Args a2;
   memset(&a2, 0, sizeof a2);
-  a2.B = c.B; a2.q = c.q; a2.pk = p->pk; a2.pk64 = c.k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
+  a2.B = c.B; a2.q = c.q; a2.io64 = c.io64; a2.pk = p->pk; a2.pk64 = c.k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
   a2.Gc = p->Gc; a2.hc = p->hc; a2.gc64 = c.k1d; a2.dt = c.dt; a2.damping = c.damping; a2.dq = p->conv_dq; a2.integrate = 1;
   a2.status = c.track ? p->conv_status : status;
   a2.warm = p->warm; a2.skip = p->conv_done; a2.gate = p->conv_count + 2;
@@ -661,16 +663,20 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   const PHeader& h = p->h;
   rc = ws_acquire(p, st);
   if (rc) return rc;
-  if ((size_t)B > p->conv_B) {
+  // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
+  const int elem = c.io64 ? 8 : 4;
+  if ((size_t)B > p->conv_B || elem > p->conv_elem) {
     conv_graph_drop(p);   // the cached graph captured the old buffers
+    const size_t nb = std::max((size_t)B, p->conv_B);
+    const int es = std::max(elem, p->conv_elem);
     cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_cursor); cudaFree(p->conv_step); cudaFree(p->conv_status);
-    p->conv_done = p->conv_cursor = p->conv_step = p->conv_status = nullptr; p->conv_dq = nullptr; p->conv_B = 0;
-    CUDA_OK(cudaMalloc(&p->conv_done, sizeof(int32_t) * (size_t)B));
-    CUDA_OK(cudaMalloc(&p->conv_dq, sizeof(float) * (size_t)B * h.nv));
-    CUDA_OK(cudaMalloc(&p->conv_cursor, sizeof(int32_t) * (size_t)B));
-    CUDA_OK(cudaMalloc(&p->conv_step, sizeof(int32_t) * (size_t)B));
-    CUDA_OK(cudaMalloc(&p->conv_status, sizeof(int32_t) * (size_t)B));
-    p->conv_B = (size_t)B;
+    p->conv_done = p->conv_cursor = p->conv_step = p->conv_status = nullptr; p->conv_dq = nullptr; p->conv_B = 0; p->conv_elem = 0;
+    CUDA_OK(cudaMalloc(&p->conv_done, sizeof(int32_t) * nb));
+    CUDA_OK(cudaMalloc(&p->conv_dq, (size_t)es * nb * h.nv));
+    CUDA_OK(cudaMalloc(&p->conv_cursor, sizeof(int32_t) * nb));
+    CUDA_OK(cudaMalloc(&p->conv_step, sizeof(int32_t) * nb));
+    CUDA_OK(cudaMalloc(&p->conv_status, sizeof(int32_t) * nb));
+    p->conv_B = nb; p->conv_elem = es;
   }
   if (!p->conv_count) CUDA_OK(cudaMalloc(&p->conv_count, 4 * sizeof(int)));
   if (!p->conv_host) CUDA_OK(cudaMallocHost(&p->conv_host, 4 * sizeof(int)));
@@ -683,7 +689,7 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
     key.B = B; key.max_iters = c.max_iters; key.check_every = 0; key.dt = c.dt; key.pos = c.pos; key.ori = c.ori; key.damping = c.damping;
     key.q = c.q; key.ft = c.in->frame_targets; key.pt = c.in->posture_targets; key.ct = c.in->com_targets; key.iters = c.iters; key.status = c.status;
     key.pb = c.in->posture_batched; key.k1d = c.k1d;
-    key.track = c.track; key.T = c.T; key.lengths = c.lengths; key.q_traj = c.q_traj;
+    key.track = c.track; key.T = c.T; key.lengths = c.lengths; key.q_traj = c.q_traj; key.io64 = c.io64;
     {
       std::lock_guard<std::mutex> l2(g_conv_mu);
       for (auto& e : g_conv) if (e.first == p) cg = e.second;
@@ -769,10 +775,10 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   return ws_release(p, st, BIK_OK);
 }
 
-extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
-                            float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, double dt, double damping, int max_iters, double pos_threshold,
+                           double ori_threshold, int check_every, int32_t* iters, int32_t* status, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, 0);
+  int rc = check_inputs(cp, in, false, io64);
   if (rc) return rc;
   if (!q || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (check_every < 1) check_every = 1;
@@ -780,18 +786,26 @@ extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_in
   ConvCall c;
   memset(&c, 0, sizeof c);
   c.B = B; c.T = 1; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
-  c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, false);
+  c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, io64 != 0); c.io64 = io64 != 0;
   return converge_run(p, c, check_every, nullptr, static_cast<cudaStream_t>(stream));
+}
+extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
+                            float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
+}
+extern "C" int bik_converge64(const bik_problem* cp, int B, double* q, const bik_inputs* in, double dt, double damping, int max_iters,
+                              double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
 }
 
 // The examples' outer loop: for each frame of a target sequence, the bik_converge loop, every instance on its own cursor.
 // One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
 // moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
-extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
-                         int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
-                         int32_t* passes, void* stream) {
+static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
+                        int max_iters, double pos_threshold, double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status,
+                        int32_t* passes, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, 0);
+  int rc = check_inputs(cp, in, false, io64);
   if (rc) return rc;
   if (!q || !q_traj || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (T < 1) return bik_fail(BIK_ERR_INVALID, "T must be at least 1");
@@ -809,8 +823,21 @@ extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bi
   ConvCall c;
   memset(&c, 0, sizeof c);
   c.B = B; c.T = T; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
-  c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = true; c.k1d = k1_double(p, damping, false);
+  c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = true; c.k1d = k1_double(p, damping, io64 != 0);
+  c.io64 = io64 != 0;
   return converge_run(p, c, check_every, passes, st);
+}
+extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
+                         int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
+                         int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 0,
+                      stream);
+}
+extern "C" int bik_track64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
+                           int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
+                           int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 1,
+                      stream);
 }
 
 // Host-buffer variant: device staging lives in the problem (separate allocations).  The batch is cut into chunks that flow

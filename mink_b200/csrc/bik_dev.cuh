@@ -103,8 +103,9 @@ struct bik_problem {
   std::vector<cudaEvent_t> hev;
   // bik_converge state
   size_t conv_B = 0;
+  int conv_elem = 0;           // bytes per conv_dq element: 4, or 8 once an fp64 call (bik_converge64 / bik_track64) needed it
   int32_t* conv_done = nullptr;
-  float* conv_dq = nullptr;
+  void* conv_dq = nullptr;     // [conv_B][nv] K2's dq of the previous pass (its warm start)
   int* conv_count = nullptr;   // device: { steps taken so far, unconverged instances }
   int* conv_host = nullptr;    // pinned mirror
   // bik_track state (the same loop, per-instance frame cursor)

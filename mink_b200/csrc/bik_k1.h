@@ -162,10 +162,18 @@ struct K1Args {
   int32_t* tstep;        // [B] steps taken in that frame; -1: no frames left (nothing is computed for the instance)
   const int32_t* lengths;   // [B] frames per instance, or null: all T
   int T;
-  float* q_traj;         // [B][T][nq]
+  void* q_traj;          // [B][T][nq], q's element type
   int32_t* traj_status;  // [B][T] or null
   signed char* warm;     // [B][max(nu,1)] K2's warm-start bytes
+  // the thresholds as the fp64 instantiation compares them (the reference tests np.linalg.norm(err[:3]) <= pos_threshold in
+  // double); fp32 callers store (double)(float) threshold here, so that the fp64 K1 they may run decides as the fp32 one
+  double pos_thr64, ori_thr64;
 };
+// the thresholds of the convergence test in the instantiation's precision
+template <typename T>
+BIK_HD T k1_pos_thr(const K1Args& a) { if constexpr (sizeof(T) == 8) return a.pos_thr64; else return T(a.pos_thr); }
+template <typename T>
+BIK_HD T k1_ori_thr(const K1Args& a) { if constexpr (sizeof(T) == 8) return a.ori_thr64; else return T(a.ori_thr); }
 
 // ---- per-warp scratch layout (elements of T) --------------------------------------------------
 BIK_HD int k1_state_stride(const PHeader& h) {  // pose (7) + CoM first moment (3) per node, odd stride
@@ -818,7 +826,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
       for (int f = 0; f < h.F; ++f) {
         const T* eb = estage + lane * K + P.frame(f).row0;
         const T pos = bik_sqrt<T>(eb[0] * eb[0] + eb[1] * eb[1] + eb[2] * eb[2]), ori = bik_sqrt<T>(eb[3] * eb[3] + eb[4] * eb[4] + eb[5] * eb[5]);
-        ok = ok && pos <= T(a.pos_thr) && ori <= T(a.ori_thr);
+        ok = ok && pos <= k1_pos_thr<T>(a) && ori <= k1_ori_thr<T>(a);
       }
       if (ok) { a.done[inst0 + lane] = 1; a.iters[inst0 + lane] = it; }
       else {
@@ -845,7 +853,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         for (int f = 0; ok && f < h.F; ++f) {
           const T* eb = estage + lane * K + P.frame(f).row0;
           const T pos = bik_sqrt<T>(eb[0] * eb[0] + eb[1] * eb[1] + eb[2] * eb[2]), ori = bik_sqrt<T>(eb[3] * eb[3] + eb[4] * eb[4] + eb[5] * eb[5]);
-          ok = pos <= T(a.pos_thr) && ori <= T(a.ori_thr);
+          ok = pos <= k1_pos_thr<T>(a) && ori <= k1_ori_thr<T>(a);
         }
         if (ok || s >= a.conv_max) {
           const int c = a.cursor[bi];
@@ -873,11 +881,23 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
     if (lane < IPW) sflag[lane] = ended;
     BIK_SYNCWARP();
     // q_traj rows of the frames that ended (from global q: the tile's copy may already hold the next tile's rows), and a cold
-    // warm start for the next frame
-    const float* qg = reinterpret_cast<const float*>(a.q);
-    for (int k = lane; k < nvalid * nq; k += W) {
-      const int i = k / nq, c = sflag[i];
-      if (c >= 0) a.q_traj[((long long)(inst0 + i) * a.T + c) * nq + (k - i * nq)] = qg[(long long)inst0 * nq + k];
+    // warm start for the next frame.  q and q_traj are fp64 only in the fp64 instantiation (bik_track64).
+    // (two plain loops rather than one generic one: the fp32 instantiations then compile to the code they had before)
+    if constexpr (sizeof(T) == 8) {
+      if (a.in64) {
+        const double* qg = static_cast<const double*>(a.q);
+        for (int k = lane; k < nvalid * nq; k += W) {
+          const int i = k / nq, c = sflag[i];
+          if (c >= 0) static_cast<double*>(a.q_traj)[((long long)(inst0 + i) * a.T + c) * nq + (k - i * nq)] = qg[(long long)inst0 * nq + k];
+        }
+      }
+    }
+    if (sizeof(T) == 4 || !a.in64) {
+      const float* qg = reinterpret_cast<const float*>(a.q);
+      for (int k = lane; k < nvalid * nq; k += W) {
+        const int i = k / nq, c = sflag[i];
+        if (c >= 0) static_cast<float*>(a.q_traj)[((long long)(inst0 + i) * a.T + c) * nq + (k - i * nq)] = qg[(long long)inst0 * nq + k];
+      }
     }
     const int nw = h.nu > 0 ? h.nu : 1;
     for (int k = lane; k < nvalid * nw; k += W)

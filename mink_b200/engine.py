@@ -238,35 +238,32 @@ class Problem:
                  damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
                  check_every: int = 1):
         """solve_ik + integrate until every frame task is within the thresholds or max_iters steps were taken, per instance
-        (the inner loop of the reference's examples; bik_converge, fp32 buffers).  q is updated in place.
-        Returns (iters [B], status [B])."""
-        assert q.is_cuda and q.is_contiguous()
-        q32 = q if q.dtype == torch.float32 else q.float()
-        inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=torch.float32)
+        (the inner loop of the reference's examples; bik_converge for a float32 q, bik_converge64 for a float64 q, the
+        targets in q's dtype).  q is updated in place.  Returns (iters [B], status [B])."""
+        assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
+        inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
         iters = torch.zeros(B, device=q.device, dtype=torch.int32)
         status = torch.zeros(B, device=q.device, dtype=torch.int32)
-        _lib.check(self.lib.bik_converge(self.handle, B, q32.data_ptr(), C.byref(inp), float(dt), float(damping), int(max_iters),
-                                         float(pos_threshold), float(ori_threshold), int(check_every), iters.data_ptr(), status.data_ptr(),
-                                         _stream()))
-        if q32 is not q:
-            q.copy_(q32)
+        fn = self.lib.bik_converge64 if _is64(q) else self.lib.bik_converge
+        _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), float(dt), float(damping), int(max_iters), float(pos_threshold),
+                      float(ori_threshold), int(check_every), iters.data_ptr(), status.data_ptr(), _stream()))
         return iters, status
 
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
               check_every: int = 1):
-        """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track, fp32 buffers):
+        """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
+        bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
         frame_targets [B,T,F,7], com_targets [B,T,C,3]; posture targets as in `converge` (the same for every frame).
         q [B,nq] is updated in place to the end of each instance's last frame.
         Returns (q_traj [B,T,nq], iters [B,T], status [B,T], passes): rows past an instance's length hold NaN / -1 / -1;
         passes is a 0-d tensor, the number of passes the device loop ran."""
-        assert q.is_cuda and q.is_contiguous()
+        assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         m = self.model
-        q32 = q if q.dtype == torch.float32 else q.float()
         B = q.shape[0]
-        seqs = [m._rows(t, n, k, dtype=torch.float32) for t, n, k in ((frame_targets, self.F, 7), (com_targets, self.Cn, 3))
+        seqs = [m._rows(t, n, k, dtype=q.dtype) for t, n, k in ((frame_targets, self.F, 7), (com_targets, self.Cn, 3))
                 if n and t is not None]
         if not seqs:
             raise ValueError("bik_track needs frame or CoM target sequences to take the number of frames from")
@@ -274,21 +271,20 @@ class Problem:
         for s in seqs:
             if B == 0 or s.shape[0] != B * T or T < 1:
                 raise ValueError(f"target sequences must be [B={B}, T, ...] with the same T >= 1")
-        inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=torch.float32)
+        inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         ln = None
         if lengths is not None:
             ln = m._dev(lengths, torch.int32).reshape(-1)
             if ln.shape[0] != B:
                 raise ValueError(f"lengths has {ln.shape[0]} entries for a batch of {B}")
-        q_traj = torch.full((B, T, self.nq), float("nan"), device=q.device, dtype=torch.float32)
+        q_traj = torch.full((B, T, self.nq), float("nan"), device=q.device, dtype=q.dtype)
         iters = torch.full((B, T), -1, device=q.device, dtype=torch.int32)
         status = torch.full((B, T), -1, device=q.device, dtype=torch.int32)
         passes = torch.zeros(1, device=q.device, dtype=torch.int32)
-        _lib.check(self.lib.bik_track(self.handle, B, T, q32.data_ptr(), C.byref(inp), _ptr(ln), float(dt), float(damping),
-                                      int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every),
-                                      q_traj.data_ptr(), iters.data_ptr(), status.data_ptr(), passes.data_ptr(), _stream()))
-        if q32 is not q:
-            q.copy_(q32)
+        fn = self.lib.bik_track64 if _is64(q) else self.lib.bik_track
+        _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(ln), float(dt), float(damping), int(max_iters),
+                      float(pos_threshold), float(ori_threshold), int(check_every), q_traj.data_ptr(), iters.data_ptr(),
+                      status.data_ptr(), passes.data_ptr(), _stream()))
         return q_traj, iters, status, passes[0]
 
     def step_host(self, q: np.ndarray, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,

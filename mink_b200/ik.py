@@ -124,7 +124,8 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
             if every FrameTask/RelativeFrameTask: |err[:3]| <= pos_threshold and |err[3:]| <= ori_threshold: break
 
     The configuration is updated in place; returns (iters, converged): steps taken and whether the thresholds were
-    met, numpy scalars for a single configuration, [B] numpy arrays for a batch."""
+    met, numpy scalars for a single configuration, [B] numpy arrays for a batch.  A single configuration and a float64
+    batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path."""
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
@@ -154,8 +155,11 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     instance, and a task not in `targets` keeps its current target.  CUDA tensors are used where they are.  `lengths`
     ([B], each in 0..T) ends instance b's sequence after lengths[b] frames.  The configuration ends at its final q.
 
-    Returns (q_traj, iters, converged) per frame: numpy [T, nq] / [T] / [T] for a single configuration, torch CUDA
-    [B, T, nq] / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
+    Sequences take the configuration's precision: a single configuration and a float64 batch run in fp64 end to end
+    (bik_track64), a float32 batch on the fp32 fast path.
+
+    Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
+    CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
     import torch
 
     for task in targets:
@@ -172,8 +176,8 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         k = 7 if isinstance(task, FrameTask) else 3
         if hasattr(seq, "wxyz_xyz"):
             seq = seq.wxyz_xyz
-        s = seq if isinstance(seq, torch.Tensor) else torch.as_tensor(np.asarray(seq, dtype=np.float32))
-        s = s.to(device=dev, dtype=torch.float32)
+        s = seq if isinstance(seq, torch.Tensor) else torch.as_tensor(np.asarray(seq, dtype=np.float64))
+        s = s.to(device=dev, dtype=q.dtype)
         if s.ndim == 2:
             s = s.unsqueeze(0).expand(B, -1, -1)
         if s.ndim != 3 or s.shape[0] != B or s.shape[2] != k or s.shape[1] < 1:
@@ -186,7 +190,8 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         raise InvalidTarget("track_ik needs at least one FrameTask / RelativeFrameTask / ComTask target sequence")
 
     def stacked(kind, k):
-        rows = [seqs[t] if t in seqs else torch.as_tensor(np.asarray(t._target(), dtype=np.float32).reshape(-1, 1, k), device=dev).expand(B, T, k)
+        rows = [seqs[t] if t in seqs else torch.as_tensor(np.asarray(t._target(), dtype=np.float64).reshape(-1, 1, k), device=dev,
+                                                          dtype=q.dtype).expand(B, T, k)
                 for t in tasks if isinstance(t, kind)]
         return torch.stack(rows, dim=2).contiguous() if rows else None
 
@@ -207,4 +212,4 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     converged = ran & ((status & 16) == 0)
     if configuration.batched:
         return q_traj, iters, converged
-    return q_traj[0].cpu().numpy().astype(np.float64), iters[0].cpu().numpy(), converged[0].cpu().numpy()
+    return q_traj[0].cpu().numpy(), iters[0].cpu().numpy(), converged[0].cpu().numpy()

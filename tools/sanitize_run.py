@@ -1,5 +1,6 @@
 """Small invocations of every kernel path for compute-sanitizer (memcheck / racecheck): K1 packed and dense (direct + staged),
-K1 fp64, both K2 paths (small-group 32/64-bit masks, general with collision rows), fp64 entry points, bik_converge, bik_track (host-polled), bik_step_host.
+K1 fp64, both K2 paths (small-group 32/64-bit masks, general with collision rows), fp64 entry points, bik_converge, bik_track and
+bik_converge64 / bik_track64 (host-polled), bik_step_host.
 Ragged batches so that tail tiles run.  Usage:  compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os
 import sys
@@ -42,6 +43,10 @@ for name, env in (("g1", {}), ("g1", {"BIK_K2_PATH": "dense"}), ("g1", {"BIK_USE
         fts[:, 1:, :, 4:] += 1e-3 * np.arange(1, 3)[None, :, None, None]
     os.environ["BIK_CONVERGE_GRAPH"] = "0"
     prob.track(q, fts, pt, seq(ct), lengths=torch.arange(45, device="cuda:0", dtype=torch.int32) % 4, dt=dt, damping=damping,
+               max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2)
+    q64 = torch.tensor(q0, dtype=torch.float64, device="cuda:0")   # the fp64 loops, host-polled
+    prob.converge(q64, ft, pt, ct, dt=dt, damping=damping, max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2)
+    prob.track(q64, fts, pt, seq(ct), lengths=torch.arange(45, device="cuda:0", dtype=torch.int32) % 4, dt=dt, damping=damping,
                max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2)
     os.environ.pop("BIK_CONVERGE_GRAPH")
     prob.step_host(q0.astype(np.float32), ft, pt, ct, dt=dt, damping=damping, nsteps=1, integrate=True)
