@@ -61,33 +61,20 @@ __global__ void check_limits_kernel(const uint32_t* __restrict__ gimage, int B, 
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b < B) status[b] = check_limits_instance<T>(P, q + (size_t)b * P.h().nq, tol);
 }
-// bik_converge bookkeeping: one thread advances the step counter and rewinds the count of unconverged instances before K1's
-// fused test; the closing kernel marks the instances that never met the thresholds.
-__global__ void converge_tick_kernel(int* count) { count[0] += 1; count[1] = 0; }
-// count = { steps taken, unconverged instances, go }.  After K1's test of step `it`: go on iff it < max_iters and (nothing has
-// been tested yet or somebody is still unconverged); `go` gates this pass's K2 and, in graph mode, the WHILE node's next pass.
-__global__ void converge_cond_kernel(int* count, int max_iters, cudaGraphConditionalHandle handle, int use_handle) {
-  const int it = count[0], go = it < max_iters && (it == 0 || count[1] > 0);
-  count[2] = go;
+// bik_converge / bik_track bookkeeping (bik_loop.h): the per-instance reset before the loop, the one-thread tick and
+// condition around K1 of every pass (the condition also sets the WHILE node's), and the per-instance finish of converge.
+__global__ void conv_reset_kernel(int B, bool track, int T, const int32_t* __restrict__ lengths, ConvBufs s) {
+  int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) conv_reset(track, T, lengths, s, b);
+}
+__global__ void conv_tick_kernel(bool track, int* count) { conv_tick(track, count); }
+__global__ void conv_cond_kernel(bool track, int max_iters, int* count, cudaGraphConditionalHandle handle, int use_handle) {
+  const int go = conv_cond(track, max_iters, count);
   if (use_handle) cudaGraphSetConditional(handle, go ? 1u : 0u);
 }
-__global__ void converge_finish_kernel(int B, int max_iters, const int32_t* __restrict__ done, int32_t* iters, int32_t* status) {
+__global__ void conv_finish_kernel(int B, int max_iters, const int32_t* __restrict__ done, int32_t* iters, int32_t* status) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b < B && !done[b]) { iters[b] = max_iters; if (status) status[b] |= 16; }
-}
-// bik_track bookkeeping: count = { passes run, instances with frames left, go }.  Every instance starts at frame 0, step 0
-// (step -1: no frames at all).  The tick counts a pass only when the previous one left work (so that the extra passes of the
-// host-polled loop are not counted) and rewinds the count that K1's test rebuilds; `go` = somebody still has frames left.
-__global__ void track_init_kernel(int B, int T, const int32_t* __restrict__ lengths, int32_t* cursor, int32_t* step, int* count) {
-  int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b < B) { cursor[b] = 0; step[b] = (lengths ? lengths[b] : T) > 0 ? 0 : -1; }
-  if (b == 0) { count[0] = 0; count[1] = 0; count[2] = 1; }
-}
-__global__ void track_tick_kernel(int* count) { count[0] += count[2]; count[1] = 0; }
-__global__ void track_cond_kernel(int* count, cudaGraphConditionalHandle handle, int use_handle) {
-  const int go = count[1] > 0;
-  count[2] = go;
-  if (use_handle) cudaGraphSetConditional(handle, go ? 1u : 0u);
+  if (b < B) conv_finish(max_iters, done, iters, status, b);
 }
 
 // CUDA-core FMA peak, measured: 16 independent dependent-chains of fused multiply-adds per thread, enough CTAs to fill every SM.
@@ -232,27 +219,7 @@ extern "C" int bik_problem_create(const bik_model* model, const bik_task_desc* t
   if (p->k2_warps != 1 && p->k2_warps != 2 && p->k2_warps != 4 && p->k2_warps != 8) p->k2_warps = 8;
   const char* k1p = getenv("BIK_K1_PRECISION");
   p->k1_prec = k1p ? (std::string(k1p) == "f64" ? 2 : (std::string(k1p) == "f32" ? 1 : 0)) : 0;
-  // conditioning estimate for the automatic choice of K1's precision: the error e enters dq amplified by about
-  // cost / (2 sqrt(regularisation)); regularisation = damping + the smallest posture weight on a coupled dof
-  {
-    double mc = 0, mp = std::numeric_limits<double>::infinity();
-    for (int t = 0; t < ntasks; ++t) {
-      if (tasks[t].kind == BIK_TASK_POSTURE) continue;
-      const int nr = tasks[t].kind == BIK_TASK_COM ? 3 : 6;
-      for (int r = 0; r < nr; ++r) mc = std::max(mc, tasks[t].cost[r] * tasks[t].cost[r]);
-    }
-    PView P{p->image.data()};
-    const int32_t* ucols = P.i(p->h.off_ucols);
-    for (int k = 0; k < p->h.nu; ++k) {
-      const int d = ucols[k];
-      if (model->hm.node_type[model->hm.dof_node[d]] == JNT_FREE) continue;
-      double s = 0;
-      for (int t = 0; t < ntasks; ++t) if (tasks[t].kind == BIK_TASK_POSTURE) s += tasks[t].dof_cost[d] * tasks[t].dof_cost[d];
-      mp = std::min(mp, s);
-    }
-    p->max_cost2 = mc;
-    p->min_post2 = std::isfinite(mp) ? mp : 0.0;
-  }
+  p->k1cond = k1_conditioning(model->hm, p->image, tasks, ntasks);
   DeviceGuard g(model->device);
   CUDA_OK(cudaMalloc(&p->d_image, p->image.size() * 4));
   CUDA_OK(cudaMemcpy(p->d_image, p->image.data(), p->image.size() * 4, cudaMemcpyHostToDevice));
@@ -283,9 +250,7 @@ extern "C" int bik_problem_dims(const bik_problem* p, bik_dims* out) {
 static bool k1_double(const bik_problem* p, double damping, bool io64) {
   if (io64 || p->k1_prec == 2) return true;
   if (p->k1_prec == 1) return false;
-  if (p->h.npairs > 0) return true;   // contact points of nearly parallel capsules are ill-conditioned in fp32
-  const double reg = damping + p->min_post2;
-  return !(reg > 0) || p->max_cost2 / reg > 1e6;
+  return k1_auto_double(p->h, p->k1cond, damping);
 }
 extern "C" size_t bik_workspace_bytes(const bik_problem* p, int B) {
   if (!p || B <= 0) return 0;
@@ -593,44 +558,24 @@ extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* 
 // as the call's arguments do not change (the usual control loop).  BIK_CONVERGE_GRAPH=0, or any failure to build the graph,
 // falls back to a host loop that reads the device counter back every `check_every` steps.
 // bik_track (below) runs the same passes with K1 in track mode; `track` selects the mode everywhere in this driver.
-// io64: fp64 buffers (bik_converge64 / bik_track64), the fp64 K1; dt and the thresholds of fp32 calls are their float values.
-struct ConvCall {
-  int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
-  void* q_traj; int32_t *iters, *status; bool track, k1d, io64;
-};
+// The pass's arguments (ConvCall), its buffers and its bookkeeping rules are defined in bik_loop.h.
 struct ConvKey {
   int B, max_iters, check_every; double dt, pos, ori; double damping; const void *q, *ft, *pt, *ct, *iters, *status; int pb; bool k1d;
   int track, T; const void *lengths, *q_traj;
   int io64;   // a buffer freed by one precision's caller may come back at the same address for the other's
   bool operator==(const ConvKey& o) const { return memcmp(this, &o, sizeof *this) == 0; }
 };
+static ConvBufs conv_bufs(const bik_problem* p) {
+  return ConvBufs{p->pk, p->Gc, p->hc, p->conv_dq, p->warm, p->conv_done, p->conv_cursor, p->conv_step, p->conv_status, p->conv_count};
+}
 // `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
 static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
-  const bik_inputs* in = c.in;
-  if (c.track) track_tick_kernel<<<1, 1, 0, st>>>(p->conv_count);
-  else converge_tick_kernel<<<1, 1, 0, st>>>(p->conv_count);
-  K1Args a1;
-  memset(&a1, 0, sizeof a1);
-  a1.B = c.B; a1.q = c.q; a1.ftgt = in->frame_targets; a1.ptgt = in->posture_targets; a1.ctgt = in->com_targets; a1.pbatched = in->posture_batched;
-  a1.in64 = c.io64; a1.dt = c.dt; a1.pk = p->pk; a1.Gc = p->Gc; a1.hc = p->hc;
-  a1.status = c.track ? p->conv_status : status; a1.tol = 1e-6f;
-  a1.done = p->conv_done; a1.iters = c.iters; a1.not_done = p->conv_count + 1; a1.conv_it = p->conv_count; a1.conv_max = c.max_iters;
-  a1.pos_thr = (float)c.pos; a1.ori_thr = (float)c.ori; a1.pos_thr64 = c.pos; a1.ori_thr64 = c.ori;
-  if (c.track) {
-    a1.cursor = p->conv_cursor; a1.tstep = p->conv_step; a1.lengths = c.lengths; a1.T = c.T;
-    a1.q_traj = c.q_traj; a1.traj_status = status; a1.warm = p->warm;
-  }
-  int rc = bik_launch_k1(p, a1, c.k1d, st);
+  const ConvBufs s = conv_bufs(p);
+  conv_tick_kernel<<<1, 1, 0, st>>>(c.track, s.count);
+  int rc = bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st);
   if (rc) return rc;
-  if (c.track) track_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, handle, use_handle);
-  else converge_cond_kernel<<<1, 1, 0, st>>>(p->conv_count, c.max_iters, handle, use_handle);
-  K2Args a2;
-  memset(&a2, 0, sizeof a2);
-  a2.B = c.B; a2.q = c.q; a2.io64 = c.io64; a2.pk = p->pk; a2.pk64 = c.k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
-  a2.Gc = p->Gc; a2.hc = p->hc; a2.gc64 = c.k1d; a2.dt = c.dt; a2.damping = c.damping; a2.dq = p->conv_dq; a2.integrate = 1;
-  a2.status = c.track ? p->conv_status : status;
-  a2.warm = p->warm; a2.skip = p->conv_done; a2.gate = p->conv_count + 2;
-  rc = dispatch_k2(p, a2, st);
+  conv_cond_kernel<<<1, 1, 0, st>>>(c.track, c.max_iters, s.count, handle, use_handle);
+  rc = dispatch_k2(p, conv_k2_args(c, s, status), st);
   if (rc) return rc;
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
@@ -738,20 +683,14 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
       }
     }
   }
-  if (c.track) {
-    track_init_kernel<<<blocks, 128, 0, st>>>(B, c.T, c.lengths, p->conv_cursor, p->conv_step, p->conv_count);
-    CUDA_OK(cudaGetLastError());
-  } else {
-    CUDA_OK(cudaMemsetAsync(p->conv_done, 0, sizeof(int32_t) * (size_t)B, st));
-    CUDA_OK(cudaMemsetAsync(p->conv_count, 0xff, sizeof(int), st));   // step counter = -1: the first tick makes it 0
-  }
+  conv_reset_kernel<<<blocks, 128, 0, st>>>(B, c.track, c.T, c.lengths, conv_bufs(p));
+  CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaMemsetAsync(p->warm, 0, (size_t)B * (size_t)(h.nu > 0 ? h.nu : 1), st));
   if (graph_ok && cg) {
     CUDA_OK(cudaGraphLaunch(cg->exec, st));
   } else {
-    // converge: passes 0..max_iters, polled after step `it` every check_every steps; track: at most T frames of max_iters + 1
-    // passes each, polled every check_every passes
-    const long long cap = c.track ? (long long)c.T * (c.max_iters + 1) : (long long)c.max_iters + 1;
+    // converge: polled after step `it` every check_every steps; track: polled every check_every passes
+    const long long cap = conv_pass_cap(c);
     bool all_done = false;
     cudaGraphConditionalHandle none{};
     for (long long it = 0; it < cap && !all_done; ++it) {
@@ -768,8 +707,7 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   if (c.track) {
     if (passes) CUDA_OK(cudaMemcpyAsync(passes, p->conv_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   } else {
-    // instances that never met the thresholds: iters = max_iters, status bit BIK_STATUS_NOT_CONVERGED
-    converge_finish_kernel<<<blocks, 128, 0, st>>>(B, c.max_iters, p->conv_done, c.iters, c.status);
+    conv_finish_kernel<<<blocks, 128, 0, st>>>(B, c.max_iters, p->conv_done, c.iters, c.status);
     CUDA_OK(cudaGetLastError());
   }
   return ws_release(p, st, BIK_OK);

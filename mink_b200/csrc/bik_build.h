@@ -461,4 +461,37 @@ inline bool build_image(const HostModel& m, const bik_task_desc* tasks, int ntas
   return true;
 }
 
+// Conditioning estimate for the automatic choice of K1's precision: the error e enters dq amplified by about
+// cost / (2 sqrt(regularisation)); regularisation = damping + the smallest posture weight on a coupled dof.
+// max_cost2: largest squared frame / CoM task cost.  min_post2: smallest squared posture cost over the coupled dofs outside
+// free joints (0 when there is none).
+struct K1Conditioning { double max_cost2 = 0, min_post2 = 0; };
+inline K1Conditioning k1_conditioning(const HostModel& m, const std::vector<uint32_t>& image, const bik_task_desc* tasks, int ntasks) {
+  double mc = 0, mp = std::numeric_limits<double>::infinity();
+  for (int t = 0; t < ntasks; ++t) {
+    if (tasks[t].kind == BIK_TASK_POSTURE) continue;
+    const int nr = tasks[t].kind == BIK_TASK_COM ? 3 : 6;
+    for (int r = 0; r < nr; ++r) mc = std::max(mc, tasks[t].cost[r] * tasks[t].cost[r]);
+  }
+  const PHeader& h = *reinterpret_cast<const PHeader*>(image.data());
+  const int32_t* ucols = reinterpret_cast<const int32_t*>(image.data() + h.off_ucols);
+  for (int k = 0; k < h.nu; ++k) {
+    const int d = ucols[k];
+    if (m.node_type[m.dof_node[d]] == JNT_FREE) continue;
+    double s = 0;
+    for (int t = 0; t < ntasks; ++t) if (tasks[t].kind == BIK_TASK_POSTURE) s += tasks[t].dof_cost[d] * tasks[t].dof_cost[d];
+    mp = std::min(mp, s);
+  }
+  K1Conditioning k;
+  k.max_cost2 = mc;
+  k.min_post2 = std::isfinite(mp) ? mp : 0.0;
+  return k;
+}
+// Whether K1 runs in fp64 for an fp32 caller of this problem and damping (BIK_K1_PRECISION aside).
+inline bool k1_auto_double(const PHeader& h, const K1Conditioning& k, double damping) {
+  if (h.npairs > 0) return true;   // contact points of nearly parallel capsules are ill-conditioned in fp32
+  const double reg = damping + k.min_post2;
+  return !(reg > 0) || k.max_cost2 / reg > 1e6;
+}
+
 }  // namespace bik

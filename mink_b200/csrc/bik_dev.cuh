@@ -19,6 +19,7 @@
 #include "bik_build.h"
 #include "bik_ptx.cuh"
 #include "bik_k2t.h"
+#include "bik_loop.h"
 
 namespace bik {
 
@@ -79,7 +80,7 @@ struct bik_problem {
   int k2_warps = 8;       // warps per CTA of the general K2 kernel (BIK_K2_WARPS)
   int k2_dynamic = 1;     // BIK_K2_DYNAMIC=0: static tile assignment in the small-group K2
   int k1_prec = 0;        // BIK_K1_PRECISION: 0 auto (by conditioning estimate), 1 f32, 2 f64
-  double max_cost2 = 0, min_post2 = 0;   // largest squared task cost / smallest squared posture cost over the coupled, bounded dofs
+  bik::K1Conditioning k1cond;   // what the automatic choice of K1's precision rests on
   // K1 -> K2 hand-off (one caller at a time per problem)
   std::mutex mu;
   size_t ws_B = 0;

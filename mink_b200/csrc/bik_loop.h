@@ -1,0 +1,87 @@
+// bik_loop.h -- one pass of the bik_converge / bik_track loop, defined once for the driver (bik_api.cu) and the host
+// emulation (tests/host_emu).
+//
+// One pass = tick, K1 (which also tests the thresholds on the errors it has just computed), condition, K2 (gated by the
+// condition).  The driver runs the passes as the body of a CUDA-graph WHILE node, or from a host-polled loop; the emulation
+// runs them one after the other on the CPU.  Both fill K1Args / K2Args here and keep the bookkeeping rules here.
+#pragma once
+#include <string.h>
+
+#include "../../include/bik.h"
+#include "bik_k2.h"
+
+namespace bik {
+
+// The arguments of one bik_converge / bik_track call.  io64: fp64 buffers (bik_converge64 / bik_track64).  k1d: K1 runs in
+// fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.
+struct ConvCall {
+  int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
+  void* q_traj; int32_t *iters, *status; bool track, k1d, io64;
+};
+
+// The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
+// the caller's precision.  warm: [B][max(nu,1)] active-set guess.  done: [B] K2 leaves the instance alone.  cursor / step /
+// status: [B] frame each instance is on, steps taken in it (-1: no frames left) and its status (track only).
+// count = { steps taken (converge) or passes run (track), instances left, go }.
+struct ConvBufs {
+  void *pk, *Gc, *hc, *dq;
+  signed char* warm;
+  int32_t *done, *cursor, *step, *status;
+  int* count;
+};
+
+// K1 of a pass.  `status` is the call's status buffer, or null (the driver's warm-up pass before a graph capture).
+inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  const bik_inputs* in = c.in;
+  K1Args a;
+  memset(&a, 0, sizeof a);
+  a.B = c.B; a.q = c.q; a.ftgt = in->frame_targets; a.ptgt = in->posture_targets; a.ctgt = in->com_targets; a.pbatched = in->posture_batched;
+  a.in64 = c.io64; a.dt = c.dt; a.pk = s.pk; a.Gc = s.Gc; a.hc = s.hc;
+  a.status = c.track ? s.status : status; a.tol = 1e-6f;
+  a.done = s.done; a.iters = c.iters; a.not_done = s.count + 1; a.conv_it = s.count; a.conv_max = c.max_iters;
+  a.pos_thr = (float)c.pos; a.ori_thr = (float)c.ori; a.pos_thr64 = c.pos; a.ori_thr64 = c.ori;
+  if (c.track) {
+    a.cursor = s.cursor; a.tstep = s.step; a.lengths = c.lengths; a.T = c.T;
+    a.q_traj = c.q_traj; a.traj_status = status; a.warm = s.warm;
+  }
+  return a;
+}
+// K2 of a pass: solves and integrates the instances K1 left undone, and does nothing once the condition said stop.
+inline K2Args conv_k2_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  const bik_inputs* in = c.in;
+  K2Args a;
+  memset(&a, 0, sizeof a);
+  a.B = c.B; a.q = c.q; a.io64 = c.io64; a.pk = s.pk; a.pk64 = c.k1d; a.ptgt = in->posture_targets; a.pbatched = in->posture_batched;
+  a.Gc = s.Gc; a.hc = s.hc; a.gc64 = c.k1d; a.dt = c.dt; a.damping = c.damping; a.dq = s.dq; a.integrate = 1;
+  a.status = c.track ? s.status : status;
+  a.warm = s.warm; a.skip = s.done; a.gate = s.count + 2;
+  return a;
+}
+
+// Before the first pass, per instance.  converge: nobody has converged, and the step counter is -1 so that the first tick
+// makes it 0.  track: every instance starts at frame 0, step 0 (step -1: no frames at all).
+BIK_HD void conv_reset(bool track, int T, const int32_t* lengths, const ConvBufs& s, int b) {
+  if (track) { s.cursor[b] = 0; s.step[b] = (lengths ? lengths[b] : T) > 0 ? 0 : -1; }
+  else s.done[b] = 0;
+  if (b == 0) { s.count[0] = track ? 0 : -1; s.count[1] = 0; s.count[2] = 1; }
+}
+// Before K1: advance the step counter (track: count a pass only when the previous one left work, so that the extra passes of
+// the host-polled loop are not counted) and rewind the count that K1's test rebuilds.
+BIK_HD void conv_tick(bool track, int* count) { count[0] += track ? count[2] : 1; count[1] = 0; }
+// After K1's test: go on iff somebody has frames left (track), or iff step `it` < max_iters and (nothing has been tested yet
+// or somebody is still unconverged) (converge).  `go` gates this pass's K2 and the next pass.
+BIK_HD int conv_cond(bool track, int max_iters, int* count) {
+  const int it = count[0];
+  const int go = track ? count[1] > 0 : it < max_iters && (it == 0 || count[1] > 0);
+  count[2] = go;
+  return go;
+}
+// After the last pass (converge): an instance that never met the thresholds gets iters = max_iters and status bit
+// BIK_STATUS_NOT_CONVERGED.
+BIK_HD void conv_finish(int max_iters, const int32_t* done, int32_t* iters, int32_t* status, int b) {
+  if (!done[b]) { iters[b] = max_iters; if (status) status[b] |= 16; }
+}
+// Passes a host-polled loop runs at most: converge, steps 0..max_iters; track, T frames of max_iters + 1 passes each.
+inline long long conv_pass_cap(const ConvCall& c) { return c.track ? (long long)c.T * (c.max_iters + 1) : (long long)c.max_iters + 1; }
+
+}  // namespace bik

@@ -131,6 +131,38 @@ class Emu:
         dq, st, it, *_ = self.solve(q, J, e, ep, None, None, dt, damping, use_double=use_double, warm=warm, dq_inout=dq_prev)
         return dq, st, it
 
+    def _loop_inputs(self, q, ftgt, ptgt, ctgt):
+        """q and the targets in q's dtype: float64 runs the ...64 loops, anything else the fp32 ones (as engine.py picks)."""
+        t = np.float64 if np.asarray(q).dtype == np.float64 else np.float32
+        q = _as(q, t).copy(); B = q.shape[0]
+        ftgt, ptgt, ctgt = _as(ftgt, t), _as(ptgt, t), _as(ctgt, t)
+        batched = int(ptgt is not None and ptgt.size == B * self.spec.nposture * self.nq and B > 1)
+        return int(t == np.float64), q, ftgt, ptgt, ctgt, batched
+
+    def converge(self, q, ftgt, ptgt, ctgt, dt, damping, max_iters, pos_threshold, ori_threshold):
+        """The pass loop of bik_converge, or of bik_converge64 for a float64 q.  Returns (q, iters, status)."""
+        f64, q, ftgt, ptgt, ctgt, batched = self._loop_inputs(q, ftgt, ptgt, ctgt)
+        B = q.shape[0]
+        it = np.zeros(B, np.int32); st = np.zeros(B, np.int32)
+        rc = lib().emu_converge(self.h, f64, B, _vp(q), _vp(ftgt), _vp(ptgt), batched, _vp(ctgt), C.c_double(dt), C.c_double(damping),
+                                int(max_iters), C.c_double(pos_threshold), C.c_double(ori_threshold), _p(it, C.c_int32), _p(st, C.c_int32))
+        assert rc == 0, lib().emu_last_error()
+        return q, it, st
+
+    def track(self, q, ftgt, ptgt, ctgt, dt, damping, max_iters, pos_threshold, ori_threshold, lengths=None):
+        """The pass loop of bik_track, or of bik_track64 for a float64 q: ftgt [B,T,F,7], ctgt [B,T,C,3].  Returns
+        (q, q_traj, iters, status, passes); rows past an instance's length hold NaN / -1 / -1."""
+        f64, q, ftgt, ptgt, ctgt, batched = self._loop_inputs(q, ftgt, ptgt, ctgt)
+        B, T = q.shape[0], (ftgt if ftgt is not None else ctgt).shape[1]
+        q_traj = np.full((B, T, self.nq), np.nan, q.dtype)
+        it = np.full((B, T), -1, np.int32); st = np.full((B, T), -1, np.int32); passes = np.zeros(1, np.int32)
+        ln = _as(lengths, np.int32)
+        rc = lib().emu_track(self.h, f64, B, T, _vp(q), _vp(ftgt), _vp(ptgt), batched, _vp(ctgt), _p(ln, C.c_int32), C.c_double(dt),
+                             C.c_double(damping), int(max_iters), C.c_double(pos_threshold), C.c_double(ori_threshold), _vp(q_traj),
+                             _p(it, C.c_int32), _p(st, C.c_int32), _p(passes, C.c_int32))
+        assert rc == 0, lib().emu_last_error()
+        return q, q_traj, it, st, int(passes[0])
+
     def fk(self, q, frames, want_J=False, f64=False):
         t = np.float64 if f64 else np.float32
         q = _as(q, t); B = q.shape[0]

@@ -1,6 +1,6 @@
-// TEST INFRASTRUCTURE -- compiles the kernel headers (mink_b200/csrc/bik_k1.h, bik_k2.h, bik_k2t.h) for the host
-// with one lane per instance (G = W = 1) so the device math can be checked against the oracle on a
-// machine without a GPU.  Never shipped, never loaded by mink_b200/: the product path is CUDA only.
+// TEST INFRASTRUCTURE -- compiles the kernel headers (mink_b200/csrc/bik_k1.h, bik_k2.h, bik_k2t.h) and the pass loop of
+// bik_converge / bik_track (bik_loop.h) for the host with one lane per instance (G = W = 1) so the device math can be checked
+// against the oracle on a machine without a GPU.  Never shipped, never loaded by mink_b200/: the product path is CUDA only.
 #include <stdlib.h>
 #include <string.h>
 
@@ -9,6 +9,7 @@
 
 #include "../../mink_b200/csrc/bik_build.h"
 #include "../../mink_b200/csrc/bik_k2t.h"
+#include "../../mink_b200/csrc/bik_loop.h"
 
 using namespace bik;
 
@@ -18,6 +19,7 @@ extern "C" const char* emu_last_error() { return g_err.c_str(); }
 struct EmuProblem {
   std::vector<uint32_t> image;        // problem image (tasks + limits; FK visits only the nodes they need)
   std::vector<uint32_t> model_image;  // model-only image, as bik_model_create builds it (FK visits every node)
+  K1Conditioning k1cond;              // what the driver's automatic choice of K1's precision rests on
 };
 
 extern "C" void* emu_problem_create(const void* blob, size_t nbytes, const bik_task_desc* tasks, int ntasks, const bik_limit_desc* limits, int nlimits) {
@@ -26,6 +28,7 @@ extern "C" void* emu_problem_create(const void* blob, size_t nbytes, const bik_t
   EmuProblem* p = new EmuProblem;
   if (!build_image(m, tasks, ntasks, limits, nlimits, 1, &p->image, &g_err)) { delete p; return nullptr; }
   if (!build_image(m, nullptr, 0, nullptr, 0, 1, &p->model_image, &g_err)) { delete p; return nullptr; }
+  p->k1cond = k1_conditioning(m, p->image, tasks, ntasks);
   return p;
 }
 // header fields of the problem image the CPU tests pin: nv, nu, nfree, nnode, nneeded, nslots, G, nsteps, pk_stride, words32, words
@@ -70,40 +73,109 @@ extern "C" int emu_fk_jac(void* prob, int B, int f64, const void* q, const void*
   return 0;
 }
 
-// K2 (fp64 solve).  path: 1 general, 3 small-group, 8 small-group with 64-bit masks.
-// Task rows: packed (pk, pk64) or dense (J, e, ep fp32; ep may be null with ptgt set).  io64: q / ptgt / dq are fp64.
-// Packed fp32 rows with fp32 I/O take the small-group step instantiation, as in bik_step.
+// K2 (fp64 solve), one instance per tile.  path: 1 general, 3 small-group, 8 small-group with 64-bit masks.  The small-group
+// instantiation follows launch_k2t: fp64 I/O or fp64 rows take the generic form, packed fp32 rows with fp32 I/O the step form.
 template <typename M>
-static void emu_k2t(const PView& P, const K2Args& a, int B, double* tw) {
+static void emu_k2t(const PView& P, const K2Args& a, double* tw) {
   const bool step = a.pk && !a.pk64 && !a.io64;
-  for (int b = 0; b < B; ++b) {
+  for (int b = 0; b < a.B; ++b) {
     if (step) k2t_warp_tile<double, 1, 1, M, true, true>(P, a, b, tw, 0);
     else k2t_warp_tile<double, 1, 1, M>(P, a, b, tw, 0);
   }
 }
+static int emu_k2(const PView& P, const K2Args& a, int path) {
+  if (path == 3 || path == 8) {
+    const int nmax = path == 8 ? K2T_NMAX_WIDE : K2T_NMAX;
+    if (P.h().npairs != 0 || P.h().nu < 1 || P.h().nu > nmax) { g_err = "small-group path not applicable"; return -1; }
+    std::vector<double> tw(k2t_warp_bytes(P, 8, 1) / 8 + 16);
+    if (path == 3) emu_k2t<uint32_t>(P, a, tw.data());
+    else emu_k2t<uint64_t>(P, a, tw.data());
+    return 0;
+  }
+  if (path != 1) { g_err = "unknown K2 path " + std::to_string(path); return -1; }
+  std::vector<double> wsm(k2_warp_bytes(P.h(), 8) / 8 + 16);
+  for (int b = 0; b < a.B; ++b) k2_warp<double, 1, 65>(P, a, b, wsm.data(), 0);
+  return 0;
+}
+// the path a solving launch takes on the device (bik_k2_group_applies, shared memory and BIK_K2_PATH aside)
+static int emu_k2_path(const PHeader& h) {
+  if (h.npairs != 0 || h.nu < 1 || h.nu > K2T_NMAX_WIDE) return 1;
+  return h.nu <= K2T_NMAX ? 3 : 8;
+}
+
+// Task rows: packed (pk, pk64) or dense (J, e, ep fp32; ep may be null with ptgt set).  io64: q / ptgt / dq are fp64.
 extern "C" int emu_solve(void* prob, int B, int path, int io64, const void* q, const void* pk, int pk64, const float* J, const float* e, const float* ep,
                          const void* ptgt, int pbatched, const void* Gc, const void* hc, int gc64, double dt, double damping, void* dq,
                          int integrate, int32_t* status, int32_t* iters, double* H, double* c, void* lo, void* hi, signed char* warm,
                          const int32_t* skip) {
   EmuProblem* p = static_cast<EmuProblem*>(prob);
-  PView P{p->image.data()};
   K2Args a;
   memset(&a, 0, sizeof a);
   a.B = B; a.q = q; a.io64 = io64; a.pk = pk; a.pk64 = pk64; a.J = J; a.e = e; a.ep = ep; a.dense64 = 0; a.ptgt = ptgt; a.pbatched = pbatched;
   a.Gc = Gc; a.hc = hc; a.gc64 = gc64; a.dt = dt; a.damping = damping; a.dq = dq; a.integrate = integrate; a.status = status; a.iters = iters;
   a.Hout = H; a.cout = c; a.lo_out = lo; a.hi_out = hi; a.warm = warm; a.skip = skip;
-  if (path == 3 || path == 8) {
-    const int nmax = path == 8 ? K2T_NMAX_WIDE : K2T_NMAX;
-    if (P.h().npairs != 0 || P.h().nu < 1 || P.h().nu > nmax) { g_err = "small-group path not applicable"; return -1; }
-    std::vector<double> tw(k2t_warp_bytes(P, 8, 1) / 8 + 16);
-    if (path == 3) emu_k2t<uint32_t>(P, a, B, tw.data());
-    else emu_k2t<uint64_t>(P, a, B, tw.data());
-    return 0;
+  return emu_k2(PView{p->image.data()}, a, path);
+}
+
+// The pass loop of bik_converge / bik_track (bik_loop.h) on host buffers: the reset, then passes as the WHILE node runs them
+// (tick, K1, condition, K2 when the condition says go) while the condition says go.  K1 runs in fp64 exactly when the driver's
+// would (BIK_K1_PRECISION aside), K2 takes the path the device takes.
+template <typename T>
+static void emu_k1_pass(const PView& P, const K1Args& a, bool track, double* wsm) {
+  for (int b = 0; b < a.B; ++b) {
+    if (track) k1_warp_tile<T, 1, 1, true, true>(P, a, b, reinterpret_cast<T*>(wsm), 0);
+    else k1_warp_tile<T, 1, 1, true, false>(P, a, b, reinterpret_cast<T*>(wsm), 0);
   }
-  if (path != 1) { g_err = "unknown K2 path " + std::to_string(path); return -1; }
-  std::vector<double> wsm(k2_warp_bytes(P.h(), 8) / 8 + 16);
-  for (int b = 0; b < B; ++b) k2_warp<double, 1, 65>(P, a, b, wsm.data(), 0);
+}
+static int emu_loop(EmuProblem* p, ConvCall c, int32_t* passes) {
+  const PView P{p->image.data()};
+  const PHeader& h = P.h();
+  const size_t B = c.B, np = std::max(h.npairs, 1);
+  c.k1d = c.io64 || k1_auto_double(h, p->k1cond, c.damping);
+  // hand-off rows and dq sized for fp64 elements whatever the precision
+  std::vector<double> pk(B * std::max(h.pk_stride, 4)), Gc(B * np * h.nv), hc(B * np), dq(B * h.nv), wsm(k1_warp_words(h, 1) + 16);
+  std::vector<signed char> warm(B * std::max(h.nu, 1));
+  std::vector<int32_t> done(B), cursor(B), step(B), status(B);
+  int count[3];
+  const ConvBufs s{pk.data(), Gc.data(), hc.data(), dq.data(), warm.data(), done.data(), cursor.data(), step.data(), status.data(), count};
+  for (int b = 0; b < c.B; ++b) conv_reset(c.track, c.T, c.lengths, s, b);
+  const K1Args a1 = conv_k1_args(c, s, c.status);
+  const K2Args a2 = conv_k2_args(c, s, c.status);
+  const int path = emu_k2_path(h);
+  for (int go = 1; go;) {
+    conv_tick(c.track, count);
+    if (c.k1d) emu_k1_pass<double>(P, a1, c.track, wsm.data());
+    else emu_k1_pass<float>(P, a1, c.track, wsm.data());
+    go = conv_cond(c.track, c.max_iters, count);
+    if (go && emu_k2(P, a2, path)) return -1;
+  }
+  if (c.track) *passes = count[0];
+  else for (int b = 0; b < c.B; ++b) conv_finish(c.max_iters, done.data(), c.iters, c.status, b);
   return 0;
+}
+// f64 = 0: bik_converge / bik_track on fp32 buffers (dt and the thresholds are rounded to float, as their parameters are);
+// f64 = 1: bik_converge64 / bik_track64 on fp64 buffers.
+static int emu_call(void* prob, int f64, bool track, int B, int T, void* q, const void* ftgt, const void* ptgt, int pbatched, const void* ctgt,
+                    const int32_t* lengths, double dt, double damping, int max_iters, double pos, double ori, void* q_traj, int32_t* iters,
+                    int32_t* status, int32_t* passes) {
+  if (!f64) { dt = (float)dt; pos = (float)pos; ori = (float)ori; }
+  bik_inputs in;
+  memset(&in, 0, sizeof in);
+  in.q = q; in.frame_targets = ftgt; in.posture_targets = ptgt; in.com_targets = ctgt; in.posture_batched = pbatched; in.f64 = f64;
+  ConvCall c;
+  memset(&c, 0, sizeof c);
+  c.B = B; c.T = T; c.max_iters = max_iters; c.dt = dt; c.pos = pos; c.ori = ori; c.damping = damping; c.q = q; c.in = &in;
+  c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = track; c.io64 = f64 != 0;
+  return emu_loop(static_cast<EmuProblem*>(prob), c, passes);
+}
+extern "C" int emu_converge(void* prob, int f64, int B, void* q, const void* ftgt, const void* ptgt, int pbatched, const void* ctgt, double dt,
+                            double damping, int max_iters, double pos, double ori, int32_t* iters, int32_t* status) {
+  return emu_call(prob, f64, false, B, 1, q, ftgt, ptgt, pbatched, ctgt, nullptr, dt, damping, max_iters, pos, ori, nullptr, iters, status, nullptr);
+}
+extern "C" int emu_track(void* prob, int f64, int B, int T, void* q, const void* ftgt, const void* ptgt, int pbatched, const void* ctgt,
+                         const int32_t* lengths, double dt, double damping, int max_iters, double pos, double ori, void* q_traj, int32_t* iters,
+                         int32_t* status, int32_t* passes) {
+  return emu_call(prob, f64, true, B, T, q, ftgt, ptgt, pbatched, ctgt, lengths, dt, damping, max_iters, pos, ori, q_traj, iters, status, passes);
 }
 
 extern "C" int emu_fk(void* prob, int B, int f64, const void* q, const bik_frame* frames, int nframes, void* poses, void* com, void* J) {

@@ -1,5 +1,4 @@
-"""bik_converge64 / bik_track64's pass loops with the kernel headers compiled for the host (tests/host_emu/track64_emu.cpp), no GPU
-needed.
+"""bik_converge64 / bik_track64's pass loops with the kernel headers compiled for the host (tests/host_emu), no GPU needed.
 
 The fp64 loops run the fp64 K1 and K2's fp64-I/O forms on fp64 buffers, collision rows included, so they are held to the
 oracle's own bars rather than to fp32 ones: the golden converge loops with identical iteration counts and flags, track64
@@ -9,9 +8,8 @@ bit-equal to the per-frame converge64 loop, and every iteration count of a ragge
 import numpy as np
 import pytest
 
-from mink_b200.workloads import make_inputs
-from tests.helpers import load_case, task_frames
-from tests.track64_emu import Track64Emu
+from tests.emu_lib import Emu
+from tests.helpers import load_case, track_case
 
 CASES = ["ur5e", "ur5e_dls", "g1", "shadow", "spot", "g1_rel", "edge", "g1_full", "g1_hands", "ur5e_damp", "ur5e_wall",
          "iiwa", "h1", "go1", "stretch", "tidybot", "aloha", "aloha_coll", "leap"]
@@ -20,14 +18,10 @@ GOLDEN_TOL = {"spot": 1e-3, "g1_rel": 1e-4, "edge": 1e-5}
 CONV = dict(max_iters=10, pos_threshold=2e-3, ori_threshold=2e-3)
 
 
-def _emu(name):
-    wl, fm, spec, g = load_case(name)
-    return wl, fm, spec, g, Track64Emu(fm.to_blob(), spec, fm.nq, fm.nv)
-
-
 @pytest.mark.parametrize("name", CASES)
 def test_emulated_converge64_matches_golden_loops(name):
-    wl, fm, spec, g, emu = _emu(name)
+    wl, fm, spec, g = load_case(name)
+    emu = Emu(fm.to_blob(), spec, fm.nq, fm.nv)
     CB = g["conv_q"].shape[0]
     max_iters, pos, ori = int(g["conv_params"][0]), float(g["conv_params"][1]), float(g["conv_params"][2])
     ct = g["com_target"][:CB] if "com_target" in g else None
@@ -42,31 +36,10 @@ def test_emulated_converge64_matches_golden_loops(name):
     assert err <= GOLDEN_TOL.get(name, 1e-6)
 
 
-def _case(name, B, T, seed, sigma=0.3):
-    from oracle.ikoracle import Oracle
-
-    wl, fm, spec, g, emu = _emu(name)
-    orc = Oracle(fm.to_blob(), spec, fm.nq, fm.nv)
-    frames = task_frames(wl, fm)
-    fk = lambda qq: orc.fk(qq, frames)
-    inp = make_inputs(fm, wl, B, fk, seed=seed, sigma=sigma)
-    rng = np.random.default_rng(seed + 1)
-    path = np.repeat(inp["q"][:, None, :], T, axis=1)
-    frac = np.arange(1, T + 1) / T
-    for n in range(fm.nnode):
-        if int(fm.node_type[n]) >= 2:   # hinge / slide: q0 (+) (t+1)/T delta
-            path[:, :, int(fm.node_qadr[n])] += rng.normal(0.0, sigma, size=B)[:, None] * frac[None, :]
-    poses, com = fk(path.reshape(B * T, fm.nq))
-    ft = np.asarray(poses, np.float64).reshape(B, T, -1, 7)
-    ct = np.asarray(com, np.float64).reshape(B, T, -1, 3) if spec.ncom else None
-    return dict(emu=emu, orc=orc, q0=inp["q"].astype(np.float64), ft=ft, ct=ct, pt=inp["q"][:, None, :].astype(np.float64),
-                kw=dict(dt=wl["dt"], damping=wl["damping"]), B=B, T=T)
-
-
 @pytest.mark.parametrize("name", ["ur5e", "h1", "ur5e_wall", "spot"])
 def test_emulated_track64_equals_per_frame_converge64(name):
     """ur5e: small-group K2; h1: CoM trajectory; ur5e_wall: collision rows, general K2; spot: the ill-conditioned case."""
-    c = _case(name, B=64 + 5, T=6, seed=12)
+    c = track_case(name, B=64 + 5, T=6, seed=12, dtype=np.float64)
     B, T = c["B"], c["T"]
     ln = np.random.default_rng(2).integers(0, T + 1, size=B).astype(np.int32)
     ln[:3] = [0, T, 1]
@@ -92,7 +65,7 @@ def test_emulated_track64_equals_per_frame_converge64(name):
 def test_emulated_track64_against_oracle():
     """The oracle's fp64 converge loop, frame after frame, on a ragged UR5e batch: every iteration count is the same and
     q_traj is within 1e-6."""
-    c = _case("ur5e", B=200 + 3, T=8, seed=44)
+    c = track_case("ur5e", B=200 + 3, T=8, seed=44, dtype=np.float64)
     B, T = c["B"], c["T"]
     ln = np.random.default_rng(4).integers(0, T + 1, size=B).astype(np.int32)
     ln[:3] = [0, T, 1]

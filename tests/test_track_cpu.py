@@ -8,38 +8,16 @@ The pass count is deterministic: max_b sum_t (iters + 1), against sum_t max_b (i
 import numpy as np
 import pytest
 
-from mink_b200.workloads import make_inputs
-from tests.track_emu import TrackEmu
-from tests.helpers import load_case, task_frames
+from tests.helpers import track_case
 
 CONV = dict(max_iters=10, pos_threshold=2e-3, ori_threshold=2e-3)
 
 
-def _case(name, B, T, seed, sigma=0.3):
-    from oracle.ikoracle import Oracle
-
-    wl, fm, spec, g = load_case(name)
-    emu = TrackEmu(fm.to_blob(), spec, fm.nq, fm.nv)
-    orc = Oracle(fm.to_blob(), spec, fm.nq, fm.nv)
-    frames = task_frames(wl, fm)
-    fk = lambda qq: orc.fk(qq, frames)
-    inp = make_inputs(fm, wl, B, fk, seed=seed, sigma=sigma)
-    rng = np.random.default_rng(seed + 1)
-    path = np.repeat(inp["q"][:, None, :], T, axis=1)
-    frac = np.arange(1, T + 1) / T
-    for n in range(fm.nnode):
-        if int(fm.node_type[n]) >= 2:   # hinge / slide: q0 (+) (t+1)/T delta
-            path[:, :, int(fm.node_qadr[n])] += rng.normal(0.0, sigma, size=B)[:, None] * frac[None, :]
-    poses, com = fk(path.reshape(B * T, fm.nq))
-    ft = np.asarray(poses, np.float32).reshape(B, T, -1, 7)
-    ct = np.asarray(com, np.float32).reshape(B, T, -1, 3) if spec.ncom else None
-    return dict(emu=emu, orc=orc, q0=inp["q"].astype(np.float32), ft=ft, ct=ct, pt=inp["q"][:, None, :].astype(np.float32),
-                kw=dict(dt=wl["dt"], damping=wl["damping"]), B=B, T=T)
-
-
-@pytest.mark.parametrize("name", ["ur5e", "h1"])
+@pytest.mark.parametrize("name", ["ur5e", "h1", "ur5e_wall", "spot"])
 def test_emulated_track_equals_per_frame_converge(name):
-    c = _case(name, B=96 + 5, T=7, seed=12)
+    """ur5e: small-group K2; h1: CoM trajectory; ur5e_wall: collision rows, so the fp64 K1 and the general K2; spot: the
+    fp64 K1 by the conditioning estimate."""
+    c = track_case(name, B=96 + 5, T=7, seed=12, dtype=np.float32)
     B, T = c["B"], c["T"]
     ln = np.random.default_rng(2).integers(0, T + 1, size=B).astype(np.int32)
     ln[:3] = [0, T, 1]
@@ -72,7 +50,7 @@ def test_emulated_track_equals_per_frame_converge(name):
 def test_emulated_track_against_oracle():
     """Iteration counts agree with the oracle's fp64 loop on >= 99.5 % of (b, t); where an instance's counts agree up to
     frame t, q_traj[b][t] is within 1e-3."""
-    c = _case("ur5e", B=200 + 3, T=8, seed=44)
+    c = track_case("ur5e", B=200 + 3, T=8, seed=44, dtype=np.float32)
     _, q_traj, it, _, _ = c["emu"].track(c["q0"], c["ft"], c["pt"], None, **c["kw"], **CONV)
     q = c["q0"].astype(np.float64)
     q_ref, it_ref = np.zeros(q_traj.shape), np.zeros_like(it)
