@@ -145,20 +145,28 @@ int bik_launch_geometry(const void* kern, const bik_model* m, size_t smem, int t
   return BIK_OK;
 }
 
-// integrate / check_limits launches: tiled (coalesced) when the tile fits the default 48 KB of dynamic shared memory
+// bik_integrate[64] / bik_check_limits[64]: tiled (coalesced) when the tile fits the default 48 KB of dynamic shared memory
 template <typename T>
-static int launch_integrate(const uint32_t* d_image, const PHeader& h, int B, T* q, const T* dq, cudaStream_t st) {
-  const size_t smem = (size_t)TILE_INST * ((h.nq | 1) + (h.nv | 1)) * sizeof(T);
-  if (smem <= 48 * 1024) integrate_tiled_kernel<T><<<(B + TILE_INST - 1) / TILE_INST, TILE_THREADS, smem, st>>>(d_image, B, q, dq);
-  else integrate_kernel<T><<<(B + 127) / 128, 128, 0, st>>>(d_image, B, q, dq);
+static int integrate_common(const bik_model* m, int B, T* q, const T* dq, void* stream) {
+  if (!m || !q || !dq || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
+  if (B == 0) return BIK_OK;
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t smem = (size_t)TILE_INST * ((m->h.nq | 1) + (m->h.nv | 1)) * sizeof(T);
+  if (smem <= 48 * 1024) integrate_tiled_kernel<T><<<(B + TILE_INST - 1) / TILE_INST, TILE_THREADS, smem, st>>>(m->d_image, B, q, dq);
+  else integrate_kernel<T><<<(B + 127) / 128, 128, 0, st>>>(m->d_image, B, q, dq);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
 template <typename T>
-static int launch_check_limits(const uint32_t* d_image, const PHeader& h, int B, const T* q, float tol, int32_t* status, cudaStream_t st) {
-  const size_t smem = (size_t)TILE_INST * (h.nq | 1) * sizeof(T);
-  if (smem <= 48 * 1024) check_limits_tiled_kernel<T><<<(B + TILE_INST - 1) / TILE_INST, TILE_THREADS, smem, st>>>(d_image, B, q, tol, status);
-  else check_limits_kernel<T><<<(B + 127) / 128, 128, 0, st>>>(d_image, B, q, tol, status);
+static int check_limits_common(const bik_model* m, int B, const T* q, float tol, int32_t* status, void* stream) {
+  if (!m || !q || !status || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
+  if (B == 0) return BIK_OK;
+  DeviceGuard g(m->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t smem = (size_t)TILE_INST * (m->h.nq | 1) * sizeof(T);
+  if (smem <= 48 * 1024) check_limits_tiled_kernel<T><<<(B + TILE_INST - 1) / TILE_INST, TILE_THREADS, smem, st>>>(m->d_image, B, q, tol, status);
+  else check_limits_kernel<T><<<(B + 127) / 128, 128, 0, st>>>(m->d_image, B, q, tol, status);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
@@ -181,6 +189,7 @@ extern "C" int bik_model_create(const void* blob, size_t nbytes, int device, bik
   if (m->G != 0 && !valid_group(m->G)) { delete m; return bik_fail(BIK_ERR_INVALID, "BIK_K1_GROUP must be 1,2,4,8,16 or 32"); }
   m->use_tma = env_int("BIK_USE_TMA", 1);
   if (!build_image(m->hm, nullptr, 0, nullptr, 0, m->G, &m->image, &err)) { delete m; return bik_fail(BIK_ERR_UNSUPPORTED, err); }
+  memcpy(&m->h, m->image.data(), sizeof(PHeader));
   DeviceGuard g(device);
   cudaDeviceProp prop;
   CUDA_OK(cudaGetDeviceProperties(&prop, device));
@@ -226,19 +235,11 @@ extern "C" int bik_problem_create(const bik_model* model, const bik_task_desc* t
   *out = p;
   return BIK_OK;
 }
-static void conv_graph_drop(bik_problem* p);
 extern "C" void bik_problem_destroy(bik_problem* p) {
   if (!p) return;
   DeviceGuard g(p->device);
-  conv_graph_drop(p);
-  cudaFree(p->d_sched); cudaFree(p->d_image); cudaFree(p->pk); cudaFree(p->Gc); cudaFree(p->hc); cudaFree(p->warm);
-  cudaFree(p->hq); cudaFree(p->hft); cudaFree(p->hpt); cudaFree(p->hct); cudaFree(p->hdq); cudaFree(p->hst);
-  cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_count); cudaFree(p->conv_cursor); cudaFree(p->conv_step); cudaFree(p->conv_status);
-  if (p->conv_host) cudaFreeHost(p->conv_host);
-  for (int i = 0; i < 4; ++i) if (p->hs[i]) cudaStreamDestroy(p->hs[i]);
-  for (cudaEvent_t e : p->hev) cudaEventDestroy(e);
-  if (p->ws_event) cudaEventDestroy(p->ws_event);
-  delete p;
+  cudaFree(p->d_sched); cudaFree(p->d_image);
+  delete p;   // the buffer groups free themselves
 }
 extern "C" int bik_problem_dims(const bik_problem* p, bik_dims* out) {
   if (!p || !out) return bik_fail(BIK_ERR_INVALID, "null argument");
@@ -379,16 +380,16 @@ extern "C" int bik_limits_box64(const bik_problem* p, int B, const double* q, do
   return box_common(p, B, q, dt, lo, hi, 1, stream);
 }
 
-// Cross-stream ordering of the per-problem workspace (callers hold p->mu).
+// Cross-stream ordering of the per-problem hand-off (callers hold p->mu).
 static int ws_acquire(bik_problem* p, cudaStream_t st) {
-  if (p->ws_pending && p->ws_stream != st) CUDA_OK(cudaStreamWaitEvent(st, p->ws_event, 0));
+  if (p->hand.pending && p->hand.stream != st) CUDA_OK(cudaStreamWaitEvent(st, p->hand.event, 0));
   return BIK_OK;
 }
 static int ws_release(bik_problem* p, cudaStream_t st, int rc) {
   if (rc) return rc;
-  if (!p->ws_event) CUDA_OK(cudaEventCreateWithFlags(&p->ws_event, cudaEventDisableTiming));
-  CUDA_OK(cudaEventRecord(p->ws_event, st));
-  p->ws_stream = st; p->ws_pending = 1;
+  if (!p->hand.event) CUDA_OK(cudaEventCreateWithFlags(&p->hand.event, cudaEventDisableTiming));
+  CUDA_OK(cudaEventRecord(p->hand.event, st));
+  p->hand.stream = st; p->hand.pending = 1;
   return BIK_OK;
 }
 
@@ -424,70 +425,56 @@ extern "C" int bik_solve64(const bik_problem* p, int B, const double* q, const d
   return solve_common(p, B, q, J, e, e_posture, G_coll, h_coll, dt, damping, dq, status, iters, 1, stream);
 }
 
-extern "C" int bik_integrate(const bik_model* m, int B, float* q, const float* dq, void* stream) {
-  if (!m || !q || !dq || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
-  if (B == 0) return BIK_OK;
-  DeviceGuard g(m->device);
-  PHeader mh;
-  memcpy(&mh, m->image.data(), sizeof mh);
-  return launch_integrate<float>(m->d_image, mh, B, q, dq, static_cast<cudaStream_t>(stream));
-}
-extern "C" int bik_integrate64(const bik_model* m, int B, double* q, const double* dq, void* stream) {
-  if (!m || !q || !dq || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
-  if (B == 0) return BIK_OK;
-  DeviceGuard g(m->device);
-  PHeader mh;
-  memcpy(&mh, m->image.data(), sizeof mh);
-  return launch_integrate<double>(m->d_image, mh, B, q, dq, static_cast<cudaStream_t>(stream));
-}
+extern "C" int bik_integrate(const bik_model* m, int B, float* q, const float* dq, void* stream) { return integrate_common(m, B, q, dq, stream); }
+extern "C" int bik_integrate64(const bik_model* m, int B, double* q, const double* dq, void* stream) { return integrate_common(m, B, q, dq, stream); }
 extern "C" int bik_check_limits(const bik_model* m, int B, const float* q, float tol, int32_t* status, void* stream) {
-  if (!m || !q || !status || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
-  if (B == 0) return BIK_OK;
-  DeviceGuard g(m->device);
-  PHeader mh;
-  memcpy(&mh, m->image.data(), sizeof mh);
-  return launch_check_limits<float>(m->d_image, mh, B, q, tol, status, static_cast<cudaStream_t>(stream));
+  return check_limits_common(m, B, q, tol, status, stream);
 }
 extern "C" int bik_check_limits64(const bik_model* m, int B, const double* q, double tol, int32_t* status, void* stream) {
-  if (!m || !q || !status || B < 0) return bik_fail(BIK_ERR_INVALID, "null argument");
-  if (B == 0) return BIK_OK;
-  DeviceGuard g(m->device);
-  PHeader mh;
-  memcpy(&mh, m->image.data(), sizeof mh);
-  return launch_check_limits<double>(m->d_image, mh, B, q, (float)tol, status, static_cast<cudaStream_t>(stream));
+  return check_limits_common(m, B, q, (float)tol, status, stream);
 }
 
-// K1 -> K2 hand-off buffers, sized for fp64 elements once a problem has needed them.
-static int ensure_workspace(bik_problem* p, int B, int elem) {
-  if ((size_t)B <= p->ws_B && elem <= p->ws_elem) return BIK_OK;
-  const PHeader& h = p->h;
-  // the buffers may still be in use by work enqueued earlier on some stream
-  CUDA_OK(cudaDeviceSynchronize());
-  const size_t b = std::max((size_t)B, p->ws_B), es = (size_t)std::max(elem, p->ws_elem);
-  cudaFree(p->pk); cudaFree(p->Gc); cudaFree(p->hc); cudaFree(p->warm);
-  p->pk = p->Gc = p->hc = nullptr; p->warm = nullptr; p->ws_B = 0;
-  CUDA_OK(cudaMalloc(&p->pk, es * b * (size_t)std::max(h.pk_stride, 4)));
-  CUDA_OK(cudaMalloc(&p->Gc, es * b * (size_t)(h.npairs > 0 ? h.npairs : 1) * h.nv));
-  CUDA_OK(cudaMalloc(&p->hc, es * b * (size_t)(h.npairs > 0 ? h.npairs : 1)));
-  CUDA_OK(cudaMalloc(&p->warm, b * (size_t)(h.nu > 0 ? h.nu : 1)));
-  p->ws_B = b; p->ws_elem = (int)es;
+// The buffer groups of a problem (bik_dev.cuh).  Callers hold p->mu.
+int Handoff::reserve(const PHeader& h, size_t B, int elem, unsigned* moves) {
+  const HandoffSizes n = handoff_sizes(h);
+  CUDA_OK(pk.reserve(elem * B * n.pk, moves));
+  CUDA_OK(Gc.reserve(elem * B * n.Gc, moves));
+  CUDA_OK(hc.reserve(elem * B * n.hc, moves));
+  CUDA_OK(warm.reserve(B * n.warm, moves));
+  return BIK_OK;
+}
+int LoopState::reserve(const PHeader& h, size_t B, int elem, unsigned* moves) {
+  for (DevBuf* b : {&done, &cursor, &step, &status}) CUDA_OK(b->reserve(sizeof(int32_t) * B, moves));
+  CUDA_OK(dq.reserve(elem * B * h.nv, moves));
+  CUDA_OK(count.reserve(4 * sizeof(int), moves));
+  if (!host) CUDA_OK(cudaMallocHost(&host, 4 * sizeof(int)));
+  return BIK_OK;
+}
+int HostStaging::reserve(const PHeader& h, size_t B, size_t pt_elems) {
+  unsigned moves = 0;   // nothing keeps these addresses between calls
+  CUDA_OK(q.reserve(4 * B * h.nq, &moves));
+  CUDA_OK(ft.reserve(4 * B * (h.F > 0 ? h.F : 1) * 7, &moves));
+  CUDA_OK(pt.reserve(4 * (pt_elems > 0 ? pt_elems : 1), &moves));
+  CUDA_OK(ct.reserve(4 * B * (h.C > 0 ? h.C : 1) * 3, &moves));
+  CUDA_OK(dq.reserve(4 * B * h.nv, &moves));
+  CUDA_OK(st.reserve(4 * B, &moves));
   return BIK_OK;
 }
 
 // One or more solve_ik steps on device buffers: per step K1 (check_limits + FK + packed task rows + collision rows) and
-// K2 (QP + integrate).  Caller holds p->mu and has sized the workspace for `k1d ? 8 : 4`-byte elements.
+// K2 (QP + integrate).  Caller holds p->mu and has reserved the hand-off for `k1d ? 8 : 4`-byte elements.
 static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, double dt, double damping, int nsteps, int integrate,
                      void* dq, int32_t* status, int io64, bool k1d, cudaStream_t st) {
-  const PHeader& h = p->h;
   // hand-off rows [ws_off, ws_off + B): chunks of one batch may be in flight on different streams (bik_step_host)
+  const HandoffSizes n = handoff_sizes(p->h);
   const size_t es = k1d ? 8 : 4;
-  char* const pk = static_cast<char*>(p->pk) + ws_off * (size_t)std::max(h.pk_stride, 4) * es;
-  char* const Gc = static_cast<char*>(p->Gc) + ws_off * (size_t)(h.npairs > 0 ? h.npairs : 1) * h.nv * es;
-  char* const hc = static_cast<char*>(p->hc) + ws_off * (size_t)(h.npairs > 0 ? h.npairs : 1) * es;
-  signed char* const warmb = p->warm + ws_off * (size_t)(h.nu > 0 ? h.nu : 1);
+  char* const pk = p->hand.pk.as<char>() + ws_off * n.pk * es;
+  char* const Gc = p->hand.Gc.as<char>() + ws_off * n.Gc * es;
+  char* const hc = p->hand.hc.as<char>() + ws_off * n.hc * es;
+  signed char* const warmb = p->hand.warm.as<signed char>() + ws_off * n.warm;
   const bool warm = nsteps > 1;   // rollouts: carry the active set (and the previous dq) from step to step
   const int phase = env_int("BIK_STEP_PHASE", 0);   // measurement aid: 1 = only K1, 2 = only K2 (on the rows the last K1 left)
-  if (warm) CUDA_OK(cudaMemsetAsync(warmb, 0, (size_t)B * (size_t)(h.nu > 0 ? h.nu : 1), st));
+  if (warm) CUDA_OK(cudaMemsetAsync(warmb, 0, (size_t)B * n.warm, st));
   for (int s = 0; s < nsteps; ++s) {
     K1Args a1;
     memset(&a1, 0, sizeof a1);
@@ -518,7 +505,7 @@ static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* 
   std::lock_guard<std::mutex> lock(p->mu);
   DeviceGuard g(p->model->device);
   const bool k1d = k1_double(p, damping, f64 != 0);
-  rc = ensure_workspace(p, B, k1d ? 8 : 4);
+  rc = p->hand.reserve(p->h, B, k1d ? 8 : 4, &p->moves);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   rc = ws_acquire(p, st);
@@ -555,18 +542,15 @@ extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* 
 // that pass are marked done and keep their q), a one-thread condition, K2 (skips the done instances, integrates the others).
 // The loop itself runs ON THE DEVICE: the passes are the body of a CUDA-graph WHILE node whose condition the condition kernel
 // sets (cudaGraphSetConditional), so the host enqueues one graph launch and never polls.  The graph is kept and reused as long
-// as the call's arguments do not change (the usual control loop).  BIK_CONVERGE_GRAPH=0, or any failure to build the graph,
+// as the call's arguments and the problem's buffers do not change (the usual control loop).  BIK_CONVERGE_GRAPH=0, or any failure to build the graph,
 // falls back to a host loop that reads the device counter back every `check_every` steps.
 // bik_track (below) runs the same passes with K1 in track mode; `track` selects the mode everywhere in this driver.
 // The pass's arguments (ConvCall), its buffers and its bookkeeping rules are defined in bik_loop.h.
-struct ConvKey {
-  int B, max_iters, check_every; double dt, pos, ori; double damping; const void *q, *ft, *pt, *ct, *iters, *status; int pb; bool k1d;
-  int track, T; const void *lengths, *q_traj;
-  int io64;   // a buffer freed by one precision's caller may come back at the same address for the other's
-  bool operator==(const ConvKey& o) const { return memcmp(this, &o, sizeof *this) == 0; }
-};
 static ConvBufs conv_bufs(const bik_problem* p) {
-  return ConvBufs{p->pk, p->Gc, p->hc, p->conv_dq, p->warm, p->conv_done, p->conv_cursor, p->conv_step, p->conv_status, p->conv_count};
+  const Handoff& w = p->hand;
+  const LoopState& l = p->loop;
+  return ConvBufs{w.pk.ptr, w.Gc.ptr, w.hc.ptr, l.dq.ptr, w.warm.as<signed char>(), l.done.as<int32_t>(), l.cursor.as<int32_t>(), l.step.as<int32_t>(),
+                  l.status.as<int32_t>(), l.count.as<int>()};
 }
 // `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
 static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
@@ -580,134 +564,95 @@ static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cud
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
-struct bik_conv_graph { ConvKey key; cudaGraph_t graph = nullptr; cudaGraphExec_t exec = nullptr; cudaStream_t cap = nullptr; };
-static std::mutex g_conv_mu;
-static std::vector<std::pair<bik_problem*, bik_conv_graph*>> g_conv;   // one cached graph per problem (heap nodes: pointers stay valid)
 
-static void conv_graph_drop(bik_problem* p) {
-  std::lock_guard<std::mutex> lock(g_conv_mu);
-  for (size_t i = 0; i < g_conv.size(); ++i)
-    if (g_conv[i].first == p) {
-      bik_conv_graph* c = g_conv[i].second;
-      if (c->exec) cudaGraphExecDestroy(c->exec);
-      if (c->graph) cudaGraphDestroy(c->graph);
-      if (c->cap) cudaStreamDestroy(c->cap);
-      delete c;
-      g_conv.erase(g_conv.begin() + i);
-      return;
+// The graph of the call: the one the problem keeps if it was built for these arguments and these buffers, else a new one
+// that replaces it.  *exec stays null when the graph cannot be built (the caller then runs the host-polled loop).
+static int conv_graph_for(bik_problem* p, const ConvCall& c, cudaStream_t st, cudaGraphExec_t* exec) {
+  ConvKey key;
+  memset(&key, 0, sizeof key);
+  key.c = c; key.c.in = nullptr;   // (every ConvCall is zero-filled before it is assigned)
+  key.in = *c.in; key.in.q = nullptr;
+  key.moves = p->moves;
+  ConvGraph& g = p->loop.graph;
+  if (g.exec && memcmp(&g.key, &key, sizeof key) == 0) { *exec = g.exec; return BIK_OK; }
+  g.drop();
+  // warm the launch-geometry cache and the tile counter outside the capture (those paths allocate / query attributes):
+  // one K1 + a K2 that skips every instance (track mode: every instance is marked as having no frames left).  The warm-up
+  // rewrites the loop state on its own stream, so an earlier call that may still be running on `st` finishes first.
+  CUDA_OK(cudaStreamSynchronize(st));
+  const ConvBufs s = conv_bufs(p);
+  bool built = false;
+  do {
+    if (cudaStreamCreateWithFlags(&g.cap, cudaStreamNonBlocking) != cudaSuccess) break;
+    cudaMemsetAsync(s.done, 1, sizeof(int32_t) * (size_t)c.B, g.cap);
+    if (c.track) cudaMemsetAsync(s.step, 0xff, sizeof(int32_t) * (size_t)c.B, g.cap);
+    cudaMemsetAsync(s.count, 0, 4 * sizeof(int), g.cap);
+    cudaGraphConditionalHandle none{};
+    if (converge_pass(p, c, nullptr, none, 0, g.cap) != BIK_OK) break;
+    if (cudaStreamSynchronize(g.cap) != cudaSuccess) break;
+    if (cudaGraphCreate(&g.graph, 0) != cudaSuccess) break;
+    cudaGraphConditionalHandle handle;
+    if (cudaGraphConditionalHandleCreate(&handle, g.graph, 1, cudaGraphCondAssignDefault) != cudaSuccess) break;
+    cudaGraphNodeParams cp2 = {cudaGraphNodeTypeConditional};
+    cp2.conditional.handle = handle; cp2.conditional.type = cudaGraphCondTypeWhile; cp2.conditional.size = 1;
+    cudaGraphNode_t node;
+    if (cudaGraphAddNode(&node, g.graph, nullptr, 0, &cp2) != cudaSuccess) break;
+    cudaGraph_t body = cp2.conditional.phGraph_out[0];
+    if (cudaStreamBeginCaptureToGraph(g.cap, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess) break;
+    const int prc = converge_pass(p, c, c.status, handle, 1, g.cap);
+    if (cudaStreamEndCapture(g.cap, nullptr) != cudaSuccess || prc != BIK_OK) break;
+    if (cudaGraphInstantiate(&g.exec, g.graph, 0) != cudaSuccess) break;
+    built = true;
+  } while (false);
+  if (built) g.key = key;
+  else { (void)cudaGetLastError(); g.drop(); }
+  *exec = g.exec;
+  return BIK_OK;
+}
+
+// The passes from the host.  converge: polled after step `it` every check_every steps; track: polled every check_every passes.
+static int conv_host_loop(bik_problem* p, const ConvCall& c, int check_every, cudaStream_t st) {
+  const long long cap = conv_pass_cap(c);
+  bool all_done = false;
+  cudaGraphConditionalHandle none{};
+  for (long long it = 0; it < cap && !all_done; ++it) {
+    int rc = converge_pass(p, c, c.status, none, 0, st);
+    if (rc) return rc;
+    const bool poll = c.track ? ((it + 1) % check_every == 0 || it + 1 == cap) : (it > 0 && (it == c.max_iters || it % check_every == 0));
+    if (poll) {
+      CUDA_OK(cudaMemcpyAsync(p->loop.host, p->loop.count.ptr, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+      CUDA_OK(cudaStreamSynchronize(st));
+      all_done = p->loop.host[1] == 0;
     }
+  }
+  return BIK_OK;
 }
 
 // The loop of bik_converge / bik_track.  Caller has validated the arguments.
 static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int32_t* passes, cudaStream_t st) {
   std::lock_guard<std::mutex> lock(p->mu);
   DeviceGuard g(p->model->device);
-  const int B = c.B;
-  int rc = ensure_workspace(p, B, c.k1d ? 8 : 4);
+  int rc = p->hand.reserve(p->h, c.B, c.k1d ? 8 : 4, &p->moves);
   if (rc) return rc;
-  const PHeader& h = p->h;
+  rc = p->loop.reserve(p->h, c.B, c.io64 ? 8 : 4, &p->moves);   // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
+  if (rc) return rc;
   rc = ws_acquire(p, st);
   if (rc) return rc;
-  // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
-  const int elem = c.io64 ? 8 : 4;
-  if ((size_t)B > p->conv_B || elem > p->conv_elem) {
-    conv_graph_drop(p);   // the cached graph captured the old buffers
-    const size_t nb = std::max((size_t)B, p->conv_B);
-    const int es = std::max(elem, p->conv_elem);
-    cudaFree(p->conv_done); cudaFree(p->conv_dq); cudaFree(p->conv_cursor); cudaFree(p->conv_step); cudaFree(p->conv_status);
-    p->conv_done = p->conv_cursor = p->conv_step = p->conv_status = nullptr; p->conv_dq = nullptr; p->conv_B = 0; p->conv_elem = 0;
-    CUDA_OK(cudaMalloc(&p->conv_done, sizeof(int32_t) * nb));
-    CUDA_OK(cudaMalloc(&p->conv_dq, (size_t)es * nb * h.nv));
-    CUDA_OK(cudaMalloc(&p->conv_cursor, sizeof(int32_t) * nb));
-    CUDA_OK(cudaMalloc(&p->conv_step, sizeof(int32_t) * nb));
-    CUDA_OK(cudaMalloc(&p->conv_status, sizeof(int32_t) * nb));
-    p->conv_B = nb; p->conv_elem = es;
-  }
-  if (!p->conv_count) CUDA_OK(cudaMalloc(&p->conv_count, 4 * sizeof(int)));
-  if (!p->conv_host) CUDA_OK(cudaMallocHost(&p->conv_host, 4 * sizeof(int)));
-  const int blocks = (B + 127) / 128;
-  bool graph_ok = env_int("BIK_CONVERGE_GRAPH", 1) != 0;
-  bik_conv_graph* cg = nullptr;
-  if (graph_ok) {
-    ConvKey key;
-    memset(&key, 0, sizeof key);
-    key.B = B; key.max_iters = c.max_iters; key.check_every = 0; key.dt = c.dt; key.pos = c.pos; key.ori = c.ori; key.damping = c.damping;
-    key.q = c.q; key.ft = c.in->frame_targets; key.pt = c.in->posture_targets; key.ct = c.in->com_targets; key.iters = c.iters; key.status = c.status;
-    key.pb = c.in->posture_batched; key.k1d = c.k1d;
-    key.track = c.track; key.T = c.T; key.lengths = c.lengths; key.q_traj = c.q_traj; key.io64 = c.io64;
-    {
-      std::lock_guard<std::mutex> l2(g_conv_mu);
-      for (auto& e : g_conv) if (e.first == p) cg = e.second;
-    }
-    if (cg && !(cg->key == key)) { conv_graph_drop(p); cg = nullptr; }
-    if (!cg) {
-      // warm the launch-geometry cache and the tile counter outside the capture (those paths allocate / query attributes):
-      // one K1 + a K2 that skips every instance (track mode: every instance is marked as having no frames left).  The warm-up
-      // rewrites the loop state on its own stream, so an earlier call that may still be running on `st` finishes first.
-      CUDA_OK(cudaStreamSynchronize(st));
-      bik_conv_graph ng;
-      ng.key = key;
-      bool built = false;
-      do {
-        if (cudaStreamCreateWithFlags(&ng.cap, cudaStreamNonBlocking) != cudaSuccess) break;
-        cudaMemsetAsync(p->conv_done, 1, sizeof(int32_t) * (size_t)B, ng.cap);
-        if (c.track) cudaMemsetAsync(p->conv_step, 0xff, sizeof(int32_t) * (size_t)B, ng.cap);
-        cudaMemsetAsync(p->conv_count, 0, 4 * sizeof(int), ng.cap);
-        cudaGraphConditionalHandle none{};
-        if (converge_pass(p, c, nullptr, none, 0, ng.cap) != BIK_OK) break;
-        if (cudaStreamSynchronize(ng.cap) != cudaSuccess) break;
-        if (cudaGraphCreate(&ng.graph, 0) != cudaSuccess) break;
-        cudaGraphConditionalHandle handle;
-        if (cudaGraphConditionalHandleCreate(&handle, ng.graph, 1, cudaGraphCondAssignDefault) != cudaSuccess) break;
-        cudaGraphNodeParams cp2 = {cudaGraphNodeTypeConditional};
-        cp2.conditional.handle = handle; cp2.conditional.type = cudaGraphCondTypeWhile; cp2.conditional.size = 1;
-        cudaGraphNode_t node;
-        if (cudaGraphAddNode(&node, ng.graph, nullptr, 0, &cp2) != cudaSuccess) break;
-        cudaGraph_t body = cp2.conditional.phGraph_out[0];
-        if (cudaStreamBeginCaptureToGraph(ng.cap, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed) != cudaSuccess) break;
-        const int prc = converge_pass(p, c, c.status, handle, 1, ng.cap);
-        if (cudaStreamEndCapture(ng.cap, nullptr) != cudaSuccess || prc != BIK_OK) break;
-        if (cudaGraphInstantiate(&ng.exec, ng.graph, 0) != cudaSuccess) break;
-        built = true;
-      } while (false);
-      if (built) {
-        std::lock_guard<std::mutex> l2(g_conv_mu);
-        cg = new bik_conv_graph(ng);
-        g_conv.push_back({p, cg});
-      } else {
-        (void)cudaGetLastError();
-        if (ng.exec) cudaGraphExecDestroy(ng.exec);
-        if (ng.graph) cudaGraphDestroy(ng.graph);
-        if (ng.cap) cudaStreamDestroy(ng.cap);
-        graph_ok = false;
-      }
-    }
-  }
-  conv_reset_kernel<<<blocks, 128, 0, st>>>(B, c.track, c.T, c.lengths, conv_bufs(p));
+  cudaGraphExec_t exec = nullptr;
+  if (env_int("BIK_CONVERGE_GRAPH", 1) != 0) rc = conv_graph_for(p, c, st, &exec);
+  if (rc) return rc;
+  const ConvBufs s = conv_bufs(p);
+  const int blocks = (c.B + 127) / 128;
+  conv_reset_kernel<<<blocks, 128, 0, st>>>(c.B, c.track, c.T, c.lengths, s);
   CUDA_OK(cudaGetLastError());
-  CUDA_OK(cudaMemsetAsync(p->warm, 0, (size_t)B * (size_t)(h.nu > 0 ? h.nu : 1), st));
-  if (graph_ok && cg) {
-    CUDA_OK(cudaGraphLaunch(cg->exec, st));
-  } else {
-    // converge: polled after step `it` every check_every steps; track: polled every check_every passes
-    const long long cap = conv_pass_cap(c);
-    bool all_done = false;
-    cudaGraphConditionalHandle none{};
-    for (long long it = 0; it < cap && !all_done; ++it) {
-      rc = converge_pass(p, c, c.status, none, 0, st);
-      if (rc) return rc;
-      const bool poll = c.track ? ((it + 1) % check_every == 0 || it + 1 == cap) : (it > 0 && (it == c.max_iters || it % check_every == 0));
-      if (poll) {
-        CUDA_OK(cudaMemcpyAsync(p->conv_host, p->conv_count, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        all_done = p->conv_host[1] == 0;
-      }
-    }
-  }
+  CUDA_OK(cudaMemsetAsync(s.warm, 0, (size_t)c.B * handoff_sizes(p->h).warm, st));
+  if (exec) CUDA_OK(cudaGraphLaunch(exec, st));
+  else rc = conv_host_loop(p, c, check_every, st);
+  if (rc) return rc;
   if (c.track) {
-    if (passes) CUDA_OK(cudaMemcpyAsync(passes, p->conv_count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (passes) CUDA_OK(cudaMemcpyAsync(passes, s.count, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   } else {
-    conv_finish_kernel<<<blocks, 128, 0, st>>>(B, c.max_iters, p->conv_done, c.iters, c.status);
+    conv_finish_kernel<<<blocks, 128, 0, st>>>(c.B, c.max_iters, s.done, c.iters, c.status);
     CUDA_OK(cudaGetLastError());
   }
   return ws_release(p, st, BIK_OK);
@@ -795,20 +740,14 @@ extern "C" int bik_step_host(const bik_problem* cp, int B, float* q_host, const 
   size_t nq = h.nq, nv = h.nv, b = (size_t)B;
   size_t pt_elems = (in->posture_batched ? b : 1) * (size_t)h.P * nq;
   std::lock_guard<std::mutex> lock(p->mu);
-  if (p->ws_pending) { CUDA_OK(cudaEventSynchronize(p->ws_event)); p->ws_pending = 0; }   // this call runs on the problem's own streams
-  if (b > p->host_B || pt_elems > p->host_pt_elems) {
-    CUDA_OK(cudaDeviceSynchronize());
-    cudaFree(p->hq); cudaFree(p->hft); cudaFree(p->hpt); cudaFree(p->hct); cudaFree(p->hdq); cudaFree(p->hst);
-    p->hq = p->hft = p->hpt = p->hct = p->hdq = nullptr; p->hst = nullptr; p->host_B = 0;
-    CUDA_OK(cudaMalloc(&p->hq, 4 * b * nq));
-    CUDA_OK(cudaMalloc(&p->hft, 4 * b * (h.F > 0 ? h.F : 1) * 7));
-    CUDA_OK(cudaMalloc(&p->hpt, 4 * (pt_elems > 0 ? pt_elems : 1)));
-    CUDA_OK(cudaMalloc(&p->hct, 4 * b * (h.C > 0 ? h.C : 1) * 3));
-    CUDA_OK(cudaMalloc(&p->hdq, 4 * b * nv));
-    CUDA_OK(cudaMalloc(&p->hst, 4 * b));
-    p->host_B = b; p->host_pt_elems = pt_elems;
-  }
-  if (!p->hs[0]) for (int i = 0; i < 4; ++i) CUDA_OK(cudaStreamCreateWithFlags(&p->hs[i], cudaStreamNonBlocking));
+  if (p->hand.pending) { CUDA_OK(cudaEventSynchronize(p->hand.event)); p->hand.pending = 0; }   // this call runs on the problem's own streams
+  HostStaging& hb = p->stage;
+  rc = hb.reserve(h, b, pt_elems);
+  if (rc) return rc;
+  if (!hb.hs[0]) for (int i = 0; i < 4; ++i) CUDA_OK(cudaStreamCreateWithFlags(&hb.hs[i], cudaStreamNonBlocking));
+  float *const hq = hb.q.as<float>(), *const hft = hb.ft.as<float>(), *const hpt = hb.pt.as<float>(), *const hct = hb.ct.as<float>(),
+        *const hdq = hb.dq.as<float>();
+  int32_t* const hst = hb.st.as<int32_t>();
   // chunk plan
   std::vector<size_t> cuts;
   const int forced = env_int("BIK_HOST_CHUNKS", 0);
@@ -837,54 +776,54 @@ extern "C" int bik_step_host(const bik_problem* cp, int B, float* q_host, const 
       used += n;
     }
   }
-  while (p->hev.size() < 2 * cuts.size() + 1) { cudaEvent_t e; CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); p->hev.push_back(e); }
+  while (hb.hev.size() < 2 * cuts.size() + 1) { cudaEvent_t e; CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); hb.hev.push_back(e); }
   const bool k1d = k1_double(p, damping, false);
-  rc = ensure_workspace(p, B, k1d ? 8 : 4);   // chunks keep disjoint hand-off rows: two of them compute at the same time
+  rc = p->hand.reserve(h, b, k1d ? 8 : 4, &p->moves);   // chunks keep disjoint hand-off rows: two of them compute at the same time
   if (rc) return rc;
-  cudaStream_t s_up = p->hs[0], s_dn = p->hs[3];
+  cudaStream_t s_up = hb.hs[0], s_dn = hb.hs[3];
   size_t up = 0, down = 0;
   // BIK_HOST_TRACE=1: timed events around every stage of every chunk, printed after the call (measurement aid)
   const bool trace = env_int("BIK_HOST_TRACE", 0) != 0;
   std::vector<cudaEvent_t> tev;
   auto mark = [&](cudaStream_t st) { if (trace) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); } };
   mark(s_up);
-  if (h.P) { CUDA_OK(cudaMemcpyAsync(p->hpt, in->posture_targets, 4 * pt_elems, cudaMemcpyHostToDevice, s_up)); up += 4 * pt_elems; }
+  if (h.P) { CUDA_OK(cudaMemcpyAsync(hpt, in->posture_targets, 4 * pt_elems, cudaMemcpyHostToDevice, s_up)); up += 4 * pt_elems; }
   // every upload is enqueued first: the copy engine then streams the chunks back to back, whatever the host spends on
   // enqueuing kernels and downloads afterwards
   size_t o = 0;
   for (size_t ci = 0; ci < cuts.size(); ++ci) {
     const size_t n = cuts[ci];
-    CUDA_OK(cudaMemcpyAsync(p->hq + o * nq, q_host + o * nq, 4 * n * nq, cudaMemcpyHostToDevice, s_up)); up += 4 * n * nq;
-    if (h.F) { CUDA_OK(cudaMemcpyAsync(p->hft + o * h.F * 7, static_cast<const float*>(in->frame_targets) + o * h.F * 7, 4 * n * h.F * 7, cudaMemcpyHostToDevice, s_up)); up += 4 * n * h.F * 7; }
-    if (h.C) { CUDA_OK(cudaMemcpyAsync(p->hct + o * h.C * 3, static_cast<const float*>(in->com_targets) + o * h.C * 3, 4 * n * h.C * 3, cudaMemcpyHostToDevice, s_up)); up += 4 * n * h.C * 3; }
-    CUDA_OK(cudaEventRecord(p->hev[2 * ci], s_up));
+    CUDA_OK(cudaMemcpyAsync(hq + o * nq, q_host + o * nq, 4 * n * nq, cudaMemcpyHostToDevice, s_up)); up += 4 * n * nq;
+    if (h.F) { CUDA_OK(cudaMemcpyAsync(hft + o * h.F * 7, static_cast<const float*>(in->frame_targets) + o * h.F * 7, 4 * n * h.F * 7, cudaMemcpyHostToDevice, s_up)); up += 4 * n * h.F * 7; }
+    if (h.C) { CUDA_OK(cudaMemcpyAsync(hct + o * h.C * 3, static_cast<const float*>(in->com_targets) + o * h.C * 3, 4 * n * h.C * 3, cudaMemcpyHostToDevice, s_up)); up += 4 * n * h.C * 3; }
+    CUDA_OK(cudaEventRecord(hb.hev[2 * ci], s_up));
     mark(s_up);
     o += n;
   }
   o = 0;
   for (size_t ci = 0; ci < cuts.size(); ++ci) {
     const size_t n = cuts[ci];
-    cudaStream_t s_cmp = p->hs[1 + (ci & 1)];   // two compute streams in turn: the tail of one chunk's K2 (CTAs waiting for their
-    CUDA_OK(cudaStreamWaitEvent(s_cmp, p->hev[2 * ci], 0));   // slowest tile) is filled by the next chunk's kernels
+    cudaStream_t s_cmp = hb.hs[1 + (ci & 1)];   // two compute streams in turn: the tail of one chunk's K2 (CTAs waiting for their
+    CUDA_OK(cudaStreamWaitEvent(s_cmp, hb.hev[2 * ci], 0));   // slowest tile) is filled by the next chunk's kernels
     mark(s_cmp);
     bik_inputs din = *in;
-    din.q = p->hq + o * nq; din.frame_targets = p->hft + o * h.F * 7; din.com_targets = p->hct + o * h.C * 3;
-    din.posture_targets = in->posture_batched ? p->hpt + o * (size_t)h.P * nq : p->hpt;
-    rc = step_core(p, (int)n, o, p->hq + o * nq, &din, dt, damping, nsteps, integrate, p->hdq + o * nv, status_host ? p->hst + o : nullptr, 0, k1d, s_cmp);
+    din.q = hq + o * nq; din.frame_targets = hft + o * h.F * 7; din.com_targets = hct + o * h.C * 3;
+    din.posture_targets = in->posture_batched ? hpt + o * (size_t)h.P * nq : hpt;
+    rc = step_core(p, (int)n, o, hq + o * nq, &din, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
     if (rc) return rc;
-    CUDA_OK(cudaEventRecord(p->hev[2 * ci + 1], s_cmp));
+    CUDA_OK(cudaEventRecord(hb.hev[2 * ci + 1], s_cmp));
     mark(s_cmp);
-    CUDA_OK(cudaStreamWaitEvent(s_dn, p->hev[2 * ci + 1], 0));
+    CUDA_OK(cudaStreamWaitEvent(s_dn, hb.hev[2 * ci + 1], 0));
     mark(s_dn);
-    CUDA_OK(cudaMemcpyAsync(dq_host + o * nv, p->hdq + o * nv, 4 * n * nv, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n * nv;
-    if (integrate) { CUDA_OK(cudaMemcpyAsync(q_host + o * nq, p->hq + o * nq, 4 * n * nq, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n * nq; }
-    if (status_host) { CUDA_OK(cudaMemcpyAsync(status_host + o, p->hst + o, 4 * n, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n; }
+    CUDA_OK(cudaMemcpyAsync(dq_host + o * nv, hdq + o * nv, 4 * n * nv, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n * nv;
+    if (integrate) { CUDA_OK(cudaMemcpyAsync(q_host + o * nq, hq + o * nq, 4 * n * nq, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n * nq; }
+    if (status_host) { CUDA_OK(cudaMemcpyAsync(status_host + o, hst + o, 4 * n, cudaMemcpyDeviceToHost, s_dn)); down += 4 * n; }
     mark(s_dn);
     o += n;
   }
   CUDA_OK(cudaStreamSynchronize(s_dn));
-  CUDA_OK(cudaStreamSynchronize(p->hs[1]));
-  CUDA_OK(cudaStreamSynchronize(p->hs[2]));
+  CUDA_OK(cudaStreamSynchronize(hb.hs[1]));
+  CUDA_OK(cudaStreamSynchronize(hb.hs[2]));
   CUDA_OK(cudaStreamSynchronize(s_up));
   if (trace) {   // uploads done (one per chunk), then per chunk: compute start, end, download start, end  (ms since the call's first event)
     std::string line = "bik_step_host trace (ms): up";

@@ -66,6 +66,87 @@ struct bik_model {
   bik::HostModel hm;
   std::vector<uint32_t> image;  // model-only image (no tasks)
   uint32_t* d_image = nullptr;
+  bik::PHeader h;               // the image's header
+};
+
+// One device allocation: move-only, freed with its owner (whose destroy function selects the device).
+struct DevBuf {
+  void* ptr = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : ptr(o.ptr), bytes(o.bytes) { o.ptr = nullptr; o.bytes = 0; }
+  ~DevBuf() { cudaFree(ptr); }
+  // Grow-only, contents not kept.  A larger request moves the allocation: work enqueued earlier on some stream may still
+  // use the old one, so the device is idle first, and *moves is counted up before the old one is freed.
+  cudaError_t reserve(size_t n, unsigned* moves) {
+    if (n <= bytes) return cudaSuccess;
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) return e;
+    ++*moves;
+    cudaFree(ptr);
+    ptr = nullptr; bytes = 0;
+    e = cudaMalloc(&ptr, n);
+    if (e == cudaSuccess) bytes = n;
+    return e;
+  }
+  template <typename T> T* as() const { return static_cast<T*>(ptr); }
+};
+
+// K1 -> K2 hand-off (bik_loop.h: handoff_sizes), 4- or 8-byte elements by K1's precision.  It belongs to the problem, not to
+// a stream, as the tile counters do: a call on another stream than the previous one first waits for that call's kernels
+// (event recorded at the end of every call that uses them).
+struct Handoff {
+  DevBuf pk, Gc, hc;
+  DevBuf warm;                 // [B][nu] active-set guess carried between the steps of one bik_step call
+  cudaEvent_t event = nullptr;
+  cudaStream_t stream = nullptr;
+  int pending = 0;
+  int reserve(const bik::PHeader& h, size_t B, int elem, unsigned* moves);
+  ~Handoff() { if (event) cudaEventDestroy(event); }
+};
+
+// The cached CUDA graph of bik_converge / bik_track and the call it was built for.  The key is compared as bytes: it is
+// zero-filled before its members are assigned.
+struct ConvKey {
+  bik::ConvCall c;             // `in` cleared: the struct it points to is the caller's, its contents are in `in`
+  bik_inputs in;               // q cleared (the loop takes q from the call)
+  unsigned moves;              // bik_problem::moves when the graph captured the hand-off and loop-state addresses
+};
+struct ConvGraph {
+  ConvKey key;
+  cudaGraph_t graph = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  cudaStream_t cap = nullptr;
+  void drop() {
+    if (exec) cudaGraphExecDestroy(exec);
+    if (graph) cudaGraphDestroy(graph);
+    if (cap) cudaStreamDestroy(cap);
+    exec = nullptr; graph = nullptr; cap = nullptr;
+  }
+};
+
+// bik_converge / bik_track loop state (bik_loop.h: ConvBufs)
+struct LoopState {
+  DevBuf done;                 // [B]
+  DevBuf dq;                   // [B][nv] K2's dq of the previous pass (its warm start), 4- or 8-byte elements by the caller's precision
+  DevBuf cursor, step, status; // [B] each: bik_track's frame cursor, steps taken in that frame, status of the frame in progress
+  DevBuf count;                // device: { steps taken so far, unconverged instances, go }
+  int* host = nullptr;         // pinned mirror of count
+  ConvGraph graph;
+  int reserve(const bik::PHeader& h, size_t B, int elem, unsigned* moves);
+  ~LoopState() { graph.drop(); if (host) cudaFreeHost(host); }
+};
+
+// bik_step_host staging (fp32)
+struct HostStaging {
+  DevBuf q, ft, pt, ct, dq, st;
+  cudaStream_t hs[4] = {nullptr, nullptr, nullptr, nullptr};   // upload, compute A, compute B, download
+  std::vector<cudaEvent_t> hev;
+  int reserve(const bik::PHeader& h, size_t B, size_t pt_elems);
+  ~HostStaging() {
+    for (cudaStream_t s : hs) if (s) cudaStreamDestroy(s);
+    for (cudaEvent_t e : hev) cudaEventDestroy(e);
+  }
 };
 
 enum { BIK_SCHED_SLOTS = 8 };
@@ -81,38 +162,14 @@ struct bik_problem {
   int k2_dynamic = 1;     // BIK_K2_DYNAMIC=0: static tile assignment in the small-group K2
   int k1_prec = 0;        // BIK_K1_PRECISION: 0 auto (by conditioning estimate), 1 f32, 2 f64
   bik::K1Conditioning k1cond;   // what the automatic choice of K1's precision rests on
-  // K1 -> K2 hand-off (one caller at a time per problem)
-  std::mutex mu;
-  size_t ws_B = 0;
-  int ws_elem = 0;        // element size the hand-off buffers were sized for (4 or 8)
-  void *pk = nullptr, *Gc = nullptr, *hc = nullptr;
-  signed char* warm = nullptr;          // [B][nu] active-set guess carried between the steps of one bik_step call
-  // the hand-off buffers, tile counters and the warm start belong to the problem, not to a stream: a call on another stream
-  // than the previous one first waits for that call's kernels (event recorded at the end of every call that uses them)
-  cudaEvent_t ws_event = nullptr;
-  cudaStream_t ws_stream = nullptr;
-  int ws_pending = 0;
+  std::mutex mu;          // one caller at a time per problem
+  Handoff hand;
+  LoopState loop;
+  unsigned moves = 0;     // times a buffer of `hand` or `loop` has moved: a graph built before the last move is stale
+  HostStaging stage;
   unsigned int* d_sched = nullptr;      // BIK_SCHED_SLOTS x 32 words: {next tile, finished CTAs} per launching stream (own 128-byte line each)
   cudaStream_t sched_stream[BIK_SCHED_SLOTS];
   int n_sched = 0;
-  // bik_step_host staging
-  size_t host_B = 0;
-  float *hq = nullptr, *hft = nullptr, *hpt = nullptr, *hct = nullptr, *hdq = nullptr;
-  int32_t* hst = nullptr;
-  size_t host_pt_elems = 0;
-  cudaStream_t hs[4] = {nullptr, nullptr, nullptr, nullptr};   // upload, compute A, compute B, download
-  std::vector<cudaEvent_t> hev;
-  // bik_converge state
-  size_t conv_B = 0;
-  int conv_elem = 0;           // bytes per conv_dq element: 4, or 8 once an fp64 call (bik_converge64 / bik_track64) needed it
-  int32_t* conv_done = nullptr;
-  void* conv_dq = nullptr;     // [conv_B][nv] K2's dq of the previous pass (its warm start)
-  int* conv_count = nullptr;   // device: { steps taken so far, unconverged instances }
-  int* conv_host = nullptr;    // pinned mirror
-  // bik_track state (the same loop, per-instance frame cursor)
-  int32_t* conv_cursor = nullptr;   // [B] frame each instance is on
-  int32_t* conv_step = nullptr;     // [B] steps taken in that frame, -1 = no frames left
-  int32_t* conv_status = nullptr;   // [B] status of the frame in progress
 };
 
 // resident CTAs per SM for (kernel, dynamic smem, threads): attribute + occupancy queries run once per combination

@@ -98,8 +98,7 @@ int bik_launch_k1(const bik_problem* p, const K1Args& a, bool use_double, cudaSt
 
 template <typename T, int G>
 static int launch_fk(const bik_model* m, const FkArgs& a, cudaStream_t st) {
-  PHeader h;
-  memcpy(&h, m->image.data(), sizeof h);
+  const PHeader& h = m->h;
   constexpr int IPW = 32 / G, THREADS = 128, NW = THREADS / 32;
   const int words = sizeof(T) == 8 ? h.words : h.words32;
   size_t smem = (size_t)words * 4 + (size_t)NW * fk_warp_words(h, IPW) * sizeof(T);
@@ -113,9 +112,7 @@ static int launch_fk(const bik_model* m, const FkArgs& a, cudaStream_t st) {
 }
 template <typename T>
 static int dispatch_fk(const bik_model* m, const FkArgs& a, cudaStream_t st) {
-  PHeader mh;
-  memcpy(&mh, m->image.data(), sizeof mh);
-  switch (mh.G) {
+  switch (m->h.G) {
     case 1: return launch_fk<T, 1>(m, a, st);
     case 2: return launch_fk<T, 2>(m, a, st);
     case 4: return launch_fk<T, 4>(m, a, st);

@@ -29,6 +29,12 @@ struct ConvBufs {
   int32_t *done, *cursor, *step, *status;
   int* count;
 };
+// Per instance: elements of a pk / Gc / hc row (4 or 8 bytes each, by K1's precision) and bytes of warm.
+struct HandoffSizes { size_t pk, Gc, hc, warm; };
+inline HandoffSizes handoff_sizes(const PHeader& h) {
+  const size_t np = h.npairs > 0 ? h.npairs : 1;
+  return HandoffSizes{(size_t)(h.pk_stride > 4 ? h.pk_stride : 4), np * h.nv, np, (size_t)(h.nu > 0 ? h.nu : 1)};
+}
 
 // K1 of a pass.  `status` is the call's status buffer, or null (the driver's warm-up pass before a graph capture).
 inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {

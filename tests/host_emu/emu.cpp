@@ -130,11 +130,12 @@ static void emu_k1_pass(const PView& P, const K1Args& a, bool track, double* wsm
 static int emu_loop(EmuProblem* p, ConvCall c, int32_t* passes) {
   const PView P{p->image.data()};
   const PHeader& h = P.h();
-  const size_t B = c.B, np = std::max(h.npairs, 1);
+  const size_t B = c.B;
+  const HandoffSizes n = handoff_sizes(h);
   c.k1d = c.io64 || k1_auto_double(h, p->k1cond, c.damping);
   // hand-off rows and dq sized for fp64 elements whatever the precision
-  std::vector<double> pk(B * std::max(h.pk_stride, 4)), Gc(B * np * h.nv), hc(B * np), dq(B * h.nv), wsm(k1_warp_words(h, 1) + 16);
-  std::vector<signed char> warm(B * std::max(h.nu, 1));
+  std::vector<double> pk(B * n.pk), Gc(B * n.Gc), hc(B * n.hc), dq(B * h.nv), wsm(k1_warp_words(h, 1) + 16);
+  std::vector<signed char> warm(B * n.warm);
   std::vector<int32_t> done(B), cursor(B), step(B), status(B);
   int count[3];
   const ConvBufs s{pk.data(), Gc.data(), hc.data(), dq.data(), warm.data(), done.data(), cursor.data(), step.data(), status.data(), count};
