@@ -36,11 +36,16 @@ static int launch_k2(const bik_problem* p, const K2Args& a, cudaStream_t st) {
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
-int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) {
+void bik_k2_general_shape(const bik_problem* p, int* lanes, int* slots) {
   const int rows = p->h.nu + 1;           // rows of the augmented factor (coupled dofs + rhs): lanes x SLOTS must cover them
-  if (rows <= 8) return launch_k2<8, 1>(p, a, st);
-  if (rows <= 16) return launch_k2<16, 1>(p, a, st);
-  const int slots = (rows + 31) / 32;
+  *lanes = rows <= 8 ? 8 : (rows <= 16 ? 16 : 32);
+  *slots = (rows + *lanes - 1) / *lanes;
+}
+int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) {
+  int lanes, slots;
+  bik_k2_general_shape(p, &lanes, &slots);
+  if (lanes == 8) return launch_k2<8, 1>(p, a, st);
+  if (lanes == 16) return launch_k2<16, 1>(p, a, st);
   if (slots <= 1) return launch_k2<32, 1>(p, a, st);
   if (slots == 2) return launch_k2<32, 2>(p, a, st);
   return launch_k2<32, 3>(p, a, st);

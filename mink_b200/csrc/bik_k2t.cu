@@ -95,10 +95,11 @@ int bik_launch_k2_group(const bik_problem* p, const K2Args& a, unsigned int* sch
 const char* bik_k2_describe(const bik_problem* p, char* buf, size_t cap) {
   if (bik_k2_group_applies(p)) snprintf(buf, cap, "small-group G=%d%s", group_of(p), p->h.nu > K2T_NMAX ? " (64-bit masks)" : "");
   else {
-    const int rows = p->h.nu + 1;
-    const int lanes = rows <= 8 ? 8 : (rows <= 16 ? 16 : 32);
-    if (lanes == 32) snprintf(buf, cap, "general warp-per-problem");
-    else snprintf(buf, cap, "general %d-lanes-per-problem", lanes);
+    int lanes, slots;
+    bik_k2_general_shape(p, &lanes, &slots);
+    if (lanes < 32) snprintf(buf, cap, "general %d-lanes-per-problem", lanes);
+    else if (slots == 1) snprintf(buf, cap, "general warp-per-problem");
+    else snprintf(buf, cap, "general warp-per-problem, %d slots per lane", slots);
   }
   return buf;
 }

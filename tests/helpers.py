@@ -59,6 +59,105 @@ def track_case(name, B, T, seed, dtype, sigma=0.3):
                 kw=dict(dt=wl["dt"], damping=wl["damping"]), B=B, T=T)
 
 
+def chain_xml(n_hinge, *, free_base=False, ball=False, branch=0, collision=False, seed=0):
+    """MJCF of a serial chain of `n_hinge` limited hinges (axes cycling x, y, z; short links with small random lateral
+    offsets) ending in the site "tip".  free_base: a free joint at the root (6 leading dofs no limit bounds).  ball: one ball
+    joint in the middle of the chain (nq = nv + 1).  branch: that many limited hinges in an untasked side branch hung off the
+    middle of the chain (dofs the tip task does not couple, numbered between the chain's).  collision: a sphere on the tip
+    and a capsule half-way up, next to a floor plane and a box."""
+    rng = np.random.default_rng(seed)
+    axes = ("1 0 0", "0 1 0", "0 0 1")
+
+    def offset():
+        dx, dy = rng.uniform(-0.015, 0.015, size=2)
+        return f"{dx:.4f} {dy:.4f} 0.05"
+
+    def hinge_body(name, k):
+        return (f'<body name="{name}" pos="{offset()}"><joint name="{name}_j" type="hinge" axis="{axes[k % 3]}" range="-1.5 1.5" '
+                f'limited="true"/><geom type="capsule" size="0.01 0.02" mass="0.1" contype="0" conaffinity="0"/>')
+
+    mid = n_hinge // 2
+    body, close = "", ""
+    for i in range(n_hinge):
+        body += hinge_body(f"b{i}", i)
+        close += "</body>"
+        if i == mid and branch:
+            body += "".join(hinge_body(f"s{k}", k + 1) for k in range(branch)) + "</body>" * branch
+        if i == mid and ball:
+            body += f'<body name="ball" pos="{offset()}"><joint name="ball_j" type="ball"/><geom type="sphere" size="0.01" mass="0.1" contype="0" conaffinity="0"/>'
+            close += "</body>"
+        if i == mid and collision:
+            body += '<geom name="mid" type="capsule" fromto="0 0 0 0 0 0.05" size="0.02"/>'
+    tip = '<site name="tip" pos="0 0 0.05"/>'
+    if collision:
+        tip += '<geom name="tip_ball" type="sphere" size="0.03" pos="0 0 0.05"/>'
+    root = body + tip + close
+    if free_base:
+        root = f'<body name="base" pos="0 0 0.4"><freejoint/><geom type="box" size="0.05 0.05 0.02" mass="1"/>{root}</body>'
+    world = ('<geom name="floor" type="plane" size="5 5 0.1" pos="0 0 -0.3"/><geom name="wall" type="box" size="0.1 1 1" '
+             'pos="0.6 0 0.5"/>' if collision else "")
+    return f'<mujoco model="chain"><compiler angle="radian"/><worldbody>{world}{root}</worldbody></mujoco>'
+
+
+def chain_case(n_hinge, *, free_base=False, ball=False, branch=0, collision=False, seed=0):
+    """A synthetic chain problem (chain_xml) as the driver sees it: a 6-D frame task on the tip, a posture task, a
+    ConfigurationLimit and a VelocityLimit whose vmax differs from dof to dof (so that some bounds are active and some are
+    not), plus the collision limit of the tip sphere and the mid capsule against the floor and the box when collision=True.
+    Returns a dict with the flat model, workload, spec, the tip frame and fk(q) through the fp64 oracle."""
+    import mink_b200 as mink
+    from mink_b200._abi import LIMIT_VELOCITY
+    from oracle.ikoracle import Oracle
+
+    xml = chain_xml(n_hinge, free_base=free_base, ball=ball, branch=branch, collision=collision, seed=seed)
+    fm = mink.flatten(mink.Model.from_xml_string(xml))
+    limits = [dict(kind="configuration", gain=0.95), dict(kind="velocity", vmax=1.0)]
+    if collision:
+        limits.append(dict(kind="collision", pairs=[(["tip_ball", "mid"], ["floor", "wall"])], gain=0.85, minimum_distance=0.01,
+                           detection_distance=0.3, bound_relaxation=0.0))
+    wl = dict(robot="chain", key=None, frames=[dict(name="tip", type="site", position_cost=1.0, orientation_cost=1.0, lm_damping=1.0)],
+              posture=dict(cost=1e-2), com=None, limits=limits, dt=2e-2, damping=1e-3)
+    spec = spec_from_workload(fm, wl)
+    rng = np.random.default_rng(seed + 1000)
+    for lim in spec.limits:
+        if lim.kind == LIMIT_VELOCITY:   # 0.75 .. 12 rad/s, i.e. a bound of 0.015 .. 0.24 rad per step
+            lim.vmax = np.exp(rng.uniform(np.log(0.75), np.log(12.0), size=len(lim.dof)))
+    frames = task_frames(wl, fm)
+    orc = Oracle(fm.to_blob(), spec, fm.nq, fm.nv)
+    return dict(xml=xml, fm=fm, wl=wl, spec=spec, frames=frames, orc=orc, fk=lambda qq: orc.fk(qq, frames))
+
+
+# The chain_case problems on both sides of every switch of K2's dispatch: id -> (chain_case keyword arguments, coupled dofs
+# nu, unbounded leading dofs nfree).  nu = 8 / 9: G = 4 -> 8 lanes per problem; 32 / 33: 32-bit -> 64-bit active-set masks;
+# 64: the widest block; nu + 1 = 8, 16, 32, 64, 65: the general path's lanes per problem and slots per lane.  With collision
+# rows every dof is coupled and the general path solves.
+CHAIN_CASES = {f"n{n}": (dict(n_hinge=n), n, 0) for n in (1, 7, 8, 9, 15, 16, 31, 32, 33, 63, 64)}
+CHAIN_CASES.update({
+    "free32": (dict(n_hinge=26, free_base=True), 32, 6),
+    "free64": (dict(n_hinge=58, free_base=True), 64, 6),
+    "ball64": (dict(n_hinge=61, ball=True), 64, 0),          # nq = 65
+    "branch33": (dict(n_hinge=33, branch=31), 33, 0),        # nv = 64, the side branch is not coupled
+})
+CHAIN_CASES.update({f"coll{n}": (dict(n_hinge=n, collision=True), n, 0) for n in (31, 32, 63, 64)})
+
+
+def chain_case_by_id(cid):
+    kw, nu, nfree = CHAIN_CASES[cid]
+    return chain_case(seed=nu, **kw)
+
+
+def assert_chain_uses_top_of_block(c, nu, q, step_out):
+    """On the oracle's optimum (Oracle.step's output for q): the last coupled dof (the tip hinge, numbered last in every
+    chain layout) is at a bound in some instances and free in others, and the mean active count lies strictly between 0 and
+    nu -- so the top bit of the active-set masks and the top slot of the factor carry real work."""
+    dq, _, st, nact = step_out
+    assert not st.any()
+    lo, hi = c["orc"].box(q, c["wl"]["dt"])
+    last = c["fm"].nv - 1
+    at_bound = (np.abs(dq[:, last] - lo[:, last]) < 1e-9) | (np.abs(dq[:, last] - hi[:, last]) < 1e-9)
+    assert at_bound.any() and not at_bound.all(), at_bound.mean()
+    assert 0 < nact.mean() < nu, nact.mean()
+
+
 def quat_align(a, b):
     """Flip sign of quaternions in a (...,4) to match b's hemisphere."""
     s = np.sign(np.sum(a * b, axis=-1, keepdims=True))
