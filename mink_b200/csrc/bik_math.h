@@ -9,7 +9,8 @@
 //   se3 ljacinv, Q ..... mink/lie/se3.py:211-249
 // but the formulas are re-derived for fp32: every coefficient of the form (1 - x)/theta^k is
 // evaluated by its Maclaurin series below |theta| = 1 instead of by the cancelling closed form the
-// fp64 reference can afford (see DESIGN.md "fp32 Lie coefficients").
+// fp64 reference can afford (see DESIGN.md "fp32 Lie coefficients").  The fp64 instantiations sum
+// more terms of the same series, so that they too are accurate to the last bits below |theta| = 1.
 #pragma once
 
 #include <math.h>
@@ -142,18 +143,38 @@ template <typename T> BIK_HD V3<T> so3_log(Q4<T> q) {
 }
 
 // A(theta) = (1 - (theta/2) cot(theta/2)) / theta^2 : coefficient of [w]x^2 in both V^-1 (se3 log)
-// and the SO(3) inverse left Jacobian.  Series below theta^2 = 1 (next term ~2e-8 relative).
+// and the SO(3) inverse left Jacobian.  Series below theta^2 = 1.  Its coefficients |B_2n| / (2n)!
+// fall only by ~1/(4 pi^2) per term: six terms leave 1.6e-10 relative at theta^2 -> 1, enough for
+// fp32; fp64 takes eleven (2e-18).  The fp64 coefficients below (and those of coef_BCD) are the
+// Maclaurin coefficients in theta^2 rounded to double, from sympy's series of the closed forms.
 template <typename T> BIK_HD T coef_A(T t2) {
   if (t2 < T(1)) {
+    if constexpr (sizeof(T) == 8)
+      return T(0.08333333333333333) + t2 * (T(0.001388888888888889) + t2 * (T(3.306878306878307e-05) + t2 * (T(8.267195767195768e-07) +
+             t2 * (T(2.08767569878681e-08) + t2 * (T(5.284190138687493e-10) + t2 * (T(1.3382536530684679e-11) + t2 * (T(3.3896802963225827e-13) +
+             t2 * (T(8.586062056277845e-15) + t2 * (T(2.174868698558062e-16) + t2 * T(5.5090028283602295e-18))))))))));
     return T(1.0 / 12.0) + t2 * (T(1.0 / 720.0) + t2 * (T(1.0 / 30240.0) + t2 * (T(1.0 / 1209600.0) + t2 * (T(1.0 / 47900160.0) + t2 * T(691.0 / 1307674368000.0)))));
   }
   T th = sqrt(t2), s, c;
   bik_sincos<T>(T(0.5) * th, &s, &c);
   return (T(1) - T(0.5) * th * c / s) / t2;
 }
-// B = (th - sin th)/th^3, C = (1 - th^2/2 - cos th)/th^4, D = (2 th - 3 sin th + th cos th)/(2 th^5)
+// B = (th - sin th)/th^3, C = (1 - th^2/2 - cos th)/th^4, D = (2 th - 3 sin th + th cos th)/(2 th^5).
+// Series below theta^2 = 1: six terms for fp32 (5e-12 relative at most), nine for fp64 (5e-17).
 template <typename T> BIK_HD void coef_BCD(T t2, T* B, T* C, T* D) {
   if (t2 < T(1)) {
+    if constexpr (sizeof(T) == 8) {
+      *B = T(0.16666666666666666) + t2 * (T(-0.008333333333333333) + t2 * (T(0.0001984126984126984) + t2 * (T(-2.7557319223985893e-06) +
+           t2 * (T(2.505210838544172e-08) + t2 * (T(-1.6059043836821613e-10) + t2 * (T(7.647163731819816e-13) + t2 * (T(-2.8114572543455206e-15) +
+           t2 * T(8.22063524662433e-18))))))));
+      *C = T(-0.041666666666666664) + t2 * (T(0.001388888888888889) + t2 * (T(-2.48015873015873e-05) + t2 * (T(2.755731922398589e-07) +
+           t2 * (T(-2.08767569878681e-09) + t2 * (T(1.1470745597729725e-11) + t2 * (T(-4.779477332387385e-14) + t2 * (T(1.5619206968586225e-16) +
+           t2 * T(-4.110317623312165e-19))))))));
+      *D = T(0.008333333333333333) + t2 * (T(-0.0003968253968253968) + t2 * (T(8.267195767195768e-06) + t2 * (T(-1.0020843354176688e-07) +
+           t2 * (T(8.029521918410807e-10) + t2 * (T(-4.58829823909189e-12) + t2 * (T(1.9680200780418645e-14) + t2 * (T(-6.576508197299464e-17) +
+           t2 * T(1.7615646957052136e-19))))))));
+      return;
+    }
     *B = T(1.0 / 6.0) + t2 * (T(-1.0 / 120.0) + t2 * (T(1.0 / 5040.0) + t2 * (T(-1.0 / 362880.0) + t2 * (T(1.0 / 39916800.0) + t2 * T(-1.0 / 6227020800.0)))));
     *C = T(-1.0 / 24.0) + t2 * (T(1.0 / 720.0) + t2 * (T(-1.0 / 40320.0) + t2 * (T(1.0 / 3628800.0) + t2 * (T(-1.0 / 479001600.0) + t2 * T(1.0 / 87178291200.0)))));
     *D = T(1.0 / 120.0) + t2 * (T(-1.0 / 2520.0) + t2 * (T(1.0 / 120960.0) + t2 * (T(-1.0 / 9979200.0) + t2 * (T(1.0 / 1245404160.0) + t2 * T(-1.0 / 217945728000.0)))));

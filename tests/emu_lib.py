@@ -171,12 +171,55 @@ class Emu:
         assert lib().emu_fk(self.h, B, int(f64), _vp(q), c_frames(frames), len(frames), _vp(poses), _vp(com), _vp(J)) == 0
         return poses, com, J
 
-    def integrate(self, q, dq):
-        q = _as(q, np.float32).copy()
-        lib().emu_integrate(self.h, q.shape[0], _p(q), _p(_as(dq, np.float32)))
+    def integrate(self, q, dq, f64=False):
+        """integrate_instance<float>, or integrate_instance<double> when f64 (q and dq in that precision)."""
+        t = np.float64 if f64 else np.float32
+        q, dq = _as(q, t).copy(), _as(dq, t)
+        lib().emu_integrate(self.h, int(f64), q.shape[0], _vp(q), _vp(dq))
         return q
 
     def check_limits(self, q, tol=1e-6):
         q = _as(q, np.float32); st = np.zeros(q.shape[0], np.int32)
         lib().emu_check_limits(self.h, q.shape[0], _p(q), C.c_float(tol), _p(st, C.c_int32))
         return st
+
+
+# ---- bik_math.h's Lie layer, one function at a time ---------------------------------------------------------------------
+# Each takes fp64 arrays with leading batch dimensions, rounds them to the instantiation's type (f64=False: float) and returns
+# the results widened to fp64.
+def _lie(fn, f64, a, b, out_shape, out2=False):
+    a = np.ascontiguousarray(a, np.float64)
+    lead = a.shape[:-1]
+    n = int(np.prod(lead, dtype=np.int64))
+    b = None if b is None else np.ascontiguousarray(np.broadcast_to(b, lead + np.shape(b)[-1:]), np.float64)
+    out = np.zeros(lead + out_shape)
+    o2 = np.zeros(lead + out_shape) if out2 else None
+    assert lib().emu_lie(fn, int(f64), n, _vp(a), _vp(b), _vp(out), _vp(o2)) == 0
+    return (out, o2) if out2 else out
+
+
+def lie_coefs(t2, f64):
+    """coef_A and coef_BCD at theta^2 = t2: [..., 4] = (A, B, C, D)."""
+    return _lie(0, f64, np.asarray(t2, np.float64)[..., None], None, (4,))
+
+
+def lie_so3_log(q, f64):
+    return _lie(1, f64, q, None, (3,))
+
+
+def lie_se3_log(q, t, f64):
+    """[..., 6] = (v, w)."""
+    return _lie(2, f64, q, t, (6,))
+
+
+def lie_ljacinv_blocks(xi, f64):
+    """se3_ljacinv_blocks at xi = (v, w): (Ji, Mi), each [..., 3, 3]."""
+    return _lie(3, f64, xi, None, (3, 3), out2=True)
+
+
+def lie_quat_sub(qa, qb, f64):
+    return _lie(4, f64, qa, qb, (3,))
+
+
+def lie_quat_integrate(q, w, f64):
+    return _lie(5, f64, q, w, (4,))

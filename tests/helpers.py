@@ -99,11 +99,13 @@ def chain_xml(n_hinge, *, free_base=False, ball=False, branch=0, collision=False
     return f'<mujoco model="chain"><compiler angle="radian"/><worldbody>{world}{root}</worldbody></mujoco>'
 
 
-def chain_case(n_hinge, *, free_base=False, ball=False, branch=0, collision=False, seed=0):
+def chain_case(n_hinge, *, free_base=False, ball=False, branch=0, collision=False, relative=False, seed=0):
     """A synthetic chain problem (chain_xml) as the driver sees it: a 6-D frame task on the tip, a posture task, a
     ConfigurationLimit and a VelocityLimit whose vmax differs from dof to dof (so that some bounds are active and some are
-    not), plus the collision limit of the tip sphere and the mid capsule against the floor and the box when collision=True.
-    Returns a dict with the flat model, workload, spec, the tip frame and fk(q) through the fp64 oracle."""
+    not), plus the collision limit of the tip sphere and the mid capsule against the floor and the box when collision=True,
+    and a RelativeFrameTask of the tip in the mid-chain body when relative=True (rows 6-11; its target is the second entry
+    of the frame targets).  Returns a dict with the flat model, workload, spec, the tip frame, fk(q) through the fp64 oracle
+    and, with relative=True, rel_frames = [tip, root] of the relative task."""
     import mink_b200 as mink
     from mink_b200._abi import LIMIT_VELOCITY
     from oracle.ikoracle import Oracle
@@ -116,6 +118,9 @@ def chain_case(n_hinge, *, free_base=False, ball=False, branch=0, collision=Fals
                            detection_distance=0.3, bound_relaxation=0.0))
     wl = dict(robot="chain", key=None, frames=[dict(name="tip", type="site", position_cost=1.0, orientation_cost=1.0, lm_damping=1.0)],
               posture=dict(cost=1e-2), com=None, limits=limits, dt=2e-2, damping=1e-3)
+    if relative:
+        wl["relative_frames"] = [dict(name="tip", type="site", root_name=f"b{n_hinge // 2}", root_type="body", position_cost=1.0,
+                                      orientation_cost=1.0, lm_damping=1.0)]
     spec = spec_from_workload(fm, wl)
     rng = np.random.default_rng(seed + 1000)
     for lim in spec.limits:
@@ -123,7 +128,10 @@ def chain_case(n_hinge, *, free_base=False, ball=False, branch=0, collision=Fals
             lim.vmax = np.exp(rng.uniform(np.log(0.75), np.log(12.0), size=len(lim.dof)))
     frames = task_frames(wl, fm)
     orc = Oracle(fm.to_blob(), spec, fm.nq, fm.nv)
-    return dict(xml=xml, fm=fm, wl=wl, spec=spec, frames=frames, orc=orc, fk=lambda qq: orc.fk(qq, frames))
+    out = dict(xml=xml, fm=fm, wl=wl, spec=spec, frames=frames, orc=orc, fk=lambda qq: orc.fk(qq, frames))
+    if relative:
+        out["rel_frames"] = [fm.frame(f[k + "name"], f[k + "type"]) for f in wl["relative_frames"] for k in ("", "root_")]
+    return out
 
 
 # The chain_case problems on both sides of every switch of K2's dispatch: id -> (chain_case keyword arguments, coupled dofs
@@ -158,8 +166,87 @@ def assert_chain_uses_top_of_block(c, nu, q, step_out):
     assert 0 < nact.mean() < nu, nact.mean()
 
 
+def qmul_np(a, b):
+    """Hamilton product of (..., 4) quaternion arrays (w, x, y, z)."""
+    w1, x1, y1, z1 = np.moveaxis(np.asarray(a), -1, 0)
+    w2, x2, y2, z2 = np.moveaxis(np.asarray(b), -1, 0)
+    return np.stack([w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2, w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2,
+                     w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2], -1)
+
+
+def qrot_np(q, v):
+    """Rotate (..., 3) vectors by unit (..., 4) quaternions."""
+    u = np.asarray(q)[..., 1:]
+    t = 2 * np.cross(u, v)
+    return v + np.asarray(q)[..., :1] * t + np.cross(u, t)
+
+
+def targets_at_angle(pose, theta, offset, rng):
+    """Targets T_t = T (R, d) for poses T [B, 7] (w, x, y, z, px, py, pz): a rotation R of exactly `theta` rad about a
+    random unit axis per instance, then a body-frame translation d of length `offset` in a random direction.  The error
+    log(T^-1 T_t) of a FrameTask at T then has angle `theta`.  At theta == pi the rotation's w
+    is exactly 0, so either sign of the log is valid."""
+    pose = np.asarray(pose, np.float64)
+    B = pose.shape[0]
+    ax = rng.normal(size=(B, 3))
+    ax /= np.linalg.norm(ax, axis=1, keepdims=True)
+    d = rng.normal(size=(B, 3))
+    d *= offset / np.linalg.norm(d, axis=1, keepdims=True)
+    c, s = (0.0, 1.0) if theta == np.pi else (np.cos(theta / 2), np.sin(theta / 2))
+    rot = np.concatenate([np.full((B, 1), c), s * ax], 1)
+    return np.concatenate([qmul_np(pose[:, :4], rot), pose[:, 4:] + qrot_np(pose[:, :4], d)], 1)
+
+
 def quat_align(a, b):
     """Flip sign of quaternions in a (...,4) to match b's hemisphere."""
     s = np.sign(np.sum(a * b, axis=-1, keepdims=True))
     s[s == 0] = 1
     return a * s
+
+
+# The Lie layer's regimes (mink_b200/csrc/bik_math.h): 0 and 1e-9 (identity branch of the Jacobian, |w|^2 < 1e-10), 1e-5 (1 -/+ 1e-3)
+# on both sides of that switch, the Maclaurin series up to theta^2 = 1 with 1 -/+ 1e-6 on both sides of its switch, the closed
+# forms above it, and the log's branch flip at pi.  Offsets: the target's translation from the frame, in m.
+LIE_ANGLES = (0.0, 1e-9, 1e-5 * (1 - 1e-3), 1e-5 * (1 + 1e-3), 1e-4, 1e-3, 0.3, 0.7, 1 - 1e-6, 1 + 1e-6, 1.5, 2.5, 3.0,
+              np.pi - 1e-2, np.pi - 1e-3)
+LIE_OFFSETS = (0.0, 1e-6, 0.3)
+# chain_case keyword arguments: a hinge chain, a free base with 26 hinges, a ball joint in a 61-hinge chain, and the tip
+# relative to a mid-chain body besides the absolute tip task
+LIE_CASES = {"n7": dict(n_hinge=7), "free32": dict(n_hinge=26, free_base=True), "ball64": dict(n_hinge=61, ball=True),
+             "rel7": dict(n_hinge=7, relative=True)}
+
+
+def lie_case(cid):
+    return chain_case(seed=7, **LIE_CASES[cid])
+
+
+def lie_targets(c, q, theta, offset, rng):
+    """Frame targets [B, F, 7] at `theta` rad and `offset` m from every frame task's current pose at q (targets_at_angle),
+    the relative task's in its root frame."""
+    poses, _ = c["orc"].fk(q, c["frames"], want_com=False)
+    ft = [targets_at_angle(poses[:, 0], theta, offset, rng)]
+    if "rel_frames" in c:
+        pr, _ = c["orc"].fk(q, c["rel_frames"], want_com=False)
+        qrc = pr[:, 1, :4] * np.array([1.0, -1.0, -1.0, -1.0])
+        rel = np.concatenate([qmul_np(qrc, pr[:, 0, :4]), qrot_np(qrc, pr[:, 0, 4:] - pr[:, 1, 4:])], 1)
+        ft.append(targets_at_angle(rel, theta, offset, rng))
+    return np.stack(ft, 1)
+
+
+def lie_task_rows(c, q, ft, e_like=None):
+    """(e [B, 6F], J [B, 6F, nv]) of the frame tasks at q, ft from tests/lie_ref: the oracle's fp64 FK and body Jacobians,
+    the Lie layer in extended precision.  e_like [B, 6F], a kernel's e: see tests/lie_ref.frame_task."""
+    from tests import lie_ref
+
+    orc = c["orc"]
+    poses, _ = orc.fk(q, c["frames"], want_com=False)
+    Jb = orc.frame_jacobian(q, c["frames"])
+    sl = lambda k: None if e_like is None else e_like[:, 6 * k:6 * k + 6]
+    e, J = lie_ref.frame_task(poses[:, 0], Jb[:, 0], ft[:, 0], sl(0))
+    es, Js = [e], [J]
+    if "rel_frames" in c:
+        pr, _ = orc.fk(q, c["rel_frames"], want_com=False)
+        Jr = orc.frame_jacobian(q, c["rel_frames"])
+        e, J = lie_ref.relative_frame_task(pr[:, 0], Jr[:, 0], pr[:, 1], Jr[:, 1], ft[:, 1], sl(1))
+        es.append(e); Js.append(J)
+    return np.concatenate(es, 1), np.concatenate(Js, 1)

@@ -194,15 +194,59 @@ extern "C" int emu_fk(void* prob, int B, int f64, const void* q, const bik_frame
   return 0;
 }
 
-extern "C" int emu_integrate(void* prob, int B, float* q, const float* dq) {
-  EmuProblem* p = static_cast<EmuProblem*>(prob);
-  PView P{p->image.data()};
-  for (int b = 0; b < B; ++b) integrate_instance<float>(P, q + (size_t)b * P.h().nq, dq + (size_t)b * P.h().nv);
+// f64 = 0: integrate_instance<float> on fp32 q / dq; f64 = 1: integrate_instance<double> on fp64 q / dq.
+template <typename T>
+static void emu_integrate_t(const PView& P, int B, T* q, const T* dq) {
+  for (int b = 0; b < B; ++b) integrate_instance<T>(P, q + (size_t)b * P.h().nq, dq + (size_t)b * P.h().nv);
+}
+extern "C" int emu_integrate(void* prob, int f64, int B, void* q, const void* dq) {
+  PView P{static_cast<EmuProblem*>(prob)->image.data()};
+  if (f64) emu_integrate_t<double>(P, B, static_cast<double*>(q), static_cast<const double*>(dq));
+  else emu_integrate_t<float>(P, B, static_cast<float*>(q), static_cast<const float*>(dq));
   return 0;
 }
 extern "C" int emu_check_limits(void* prob, int B, const float* q, float tol, int32_t* status) {
   EmuProblem* p = static_cast<EmuProblem*>(prob);
   PView P{p->image.data()};
   for (int b = 0; b < B; ++b) status[b] = check_limits_instance<float>(P, q + (size_t)b * P.h().nq, tol);
+  return 0;
+}
+
+// bik_math.h's Lie layer, one function on n inputs, in float (f64 = 0) or double (f64 = 1).  Inputs and outputs are fp64
+// arrays: inputs are rounded to T on the way in (exact when the caller rounded them to T already), results widened on the way out.
+template <typename T> static Q4<T> ld_q4(const double* a) { return q4<T>(T(a[0]), T(a[1]), T(a[2]), T(a[3])); }
+template <typename T> static V3<T> ld_v3(const double* a) { return v3<T>(T(a[0]), T(a[1]), T(a[2])); }
+template <typename T> static void st_v3(V3<T> v, double* a) { a[0] = v.x; a[1] = v.y; a[2] = v.z; }
+template <typename T> static void st_m3(const M3<T>& m, double* a) { for (int i = 0; i < 9; ++i) a[i] = m.m[i]; }
+
+template <typename T>
+static void lie_t(int fn, int n, const double* a, const double* b, double* out, double* out2) {
+  for (int i = 0; i < n; ++i) {
+    if (fn == 0) {          // coefficients at theta^2 = a[i]: out[4i..] = A, B, C, D
+      T B, C, D;
+      coef_BCD<T>(T(a[i]), &B, &C, &D);
+      out[4 * i] = coef_A<T>(T(a[i])); out[4 * i + 1] = B; out[4 * i + 2] = C; out[4 * i + 3] = D;
+    } else if (fn == 1) {   // so3_log(q = a[4i..])
+      st_v3(so3_log<T>(ld_q4<T>(a + 4 * i)), out + 3 * i);
+    } else if (fn == 2) {   // se3_log(q = a[4i..], t = b[3i..]) -> (v, w)
+      V3<T> v, w;
+      se3_log<T>(ld_q4<T>(a + 4 * i), ld_v3<T>(b + 3 * i), &v, &w);
+      st_v3(v, out + 6 * i); st_v3(w, out + 6 * i + 3);
+    } else if (fn == 3) {   // se3_ljacinv_blocks(v = a[6i..], w = a[6i+3..]) -> Ji (out), Mi (out2), row major
+      M3<T> Ji, Mi;
+      se3_ljacinv_blocks<T>(ld_v3<T>(a + 6 * i), ld_v3<T>(a + 6 * i + 3), &Ji, &Mi);
+      st_m3(Ji, out + 9 * i); st_m3(Mi, out2 + 9 * i);
+    } else if (fn == 4) {   // quat_sub(qa = a[4i..], qb = b[4i..])
+      st_v3(quat_sub<T>(ld_q4<T>(a + 4 * i), ld_q4<T>(b + 4 * i)), out + 3 * i);
+    } else {                // quat_integrate(q = a[4i..], w = b[3i..])
+      Q4<T> o = quat_integrate<T>(ld_q4<T>(a + 4 * i), ld_v3<T>(b + 3 * i));
+      out[4 * i] = o.w; out[4 * i + 1] = o.x; out[4 * i + 2] = o.y; out[4 * i + 3] = o.z;
+    }
+  }
+}
+extern "C" int emu_lie(int fn, int f64, int n, const double* a, const double* b, double* out, double* out2) {
+  if (fn < 0 || fn > 5) { g_err = "unknown Lie function " + std::to_string(fn); return -1; }
+  if (f64) lie_t<double>(fn, n, a, b, out, out2);
+  else lie_t<float>(fn, n, a, b, out, out2);
   return 0;
 }
