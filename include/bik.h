@@ -49,6 +49,8 @@ typedef enum bik_status {
 #define BIK_STATUS_QP_INFEASIBLE 8u  /* inequality set inconsistent (lower > upper for a dof, or no feasible start): the
                                       * reference's solver returns None there and solve_ik asserts (solve_ik.py:103) */
 #define BIK_STATUS_NOT_CONVERGED 16u /* bik_converge: thresholds not met within max_iters */
+#define BIK_STATUS_BAD_WEIGHT    32u /* ..._weighted entry points: a task weight of the instance is outside [0, 1] or NaN; it was
+                                      * clamped to [0, 1] (NaN to 0) and the step went on with the clamped value */
 
 typedef struct bik_model bik_model;     /* flattened kinematic tree resident on one device */
 typedef struct bik_problem bik_problem; /* static task + limit layout bound to a model */
@@ -280,6 +282,39 @@ int bik_converge64(const bik_problem* problem, int B, double* q, const bik_input
 int bik_track64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths,
                 double dt, double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
                 double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+
+/* ---- per-instance task weights -----------------------------------------------------------------------------------------
+ * The entry points above with one more argument, `weights`, right after `in`: each instance scales the costs of its own frame
+ * and CoM task rows, as mink's FrameTask.set_position_cost / set_orientation_cost / ComTask.set_cost would between two
+ * solve_ik calls, without building another problem.
+ *   weights [B][K] (K = bik_dims.nrows; bik_track: [B][T][K], row t is used while the instance is on frame t), device memory,
+ *           float or double like the other inputs (bik_inputs.f64).  Rows in the stacked order of J: per FRAME /
+ *           RELATIVE_FRAME task position xyz then orientation xyz, per COM task xyz, in task order.  NULL: all ones, the
+ *           results of the unweighted entry point.
+ *   The cost of row r of instance b is cost_r * w[b][r]: it scales the row of J and e in H, c and the Levenberg-Marquardt
+ *   term mu = lm_damping ||W(-gain e)||^2 exactly as a cost does.  A weight outside [0, 1] is clamped to [0, 1], NaN to 0,
+ *   and the instance gets BIK_STATUS_BAD_WEIGHT.  PostureTask / DampingTask rows have no weights.
+ *   The convergence test of bik_converge / bik_track compares the unweighted errors with the thresholds, except that a frame
+ *   task whose three position weights are all 0 in an instance has its position error left out of that instance's test
+ *   (orientation likewise): a fully occluded target does not hold the instance for max_iters steps. */
+int bik_step_weighted(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, float dt,
+                      double damping, int nsteps, int integrate, float* dq, int32_t* status, void* stream);
+int bik_converge_weighted(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, float dt,
+                          double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every,
+                          int32_t* iters, int32_t* status, void* stream);
+int bik_track_weighted(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights,
+                       const int32_t* lengths, float dt, double damping, int max_iters, float pos_threshold,
+                       float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status, int32_t* passes,
+                       void* stream);
+int bik_step_weighted64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, double dt,
+                        double damping, int nsteps, int integrate, double* dq, int32_t* status, void* stream);
+int bik_converge_weighted64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, double dt,
+                            double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
+                            int32_t* iters, int32_t* status, void* stream);
+int bik_track_weighted64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                         const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
+                         double ori_threshold, int check_every, double* q_traj, int32_t* iters, int32_t* status,
+                         int32_t* passes, void* stream);
 
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */

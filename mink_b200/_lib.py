@@ -15,7 +15,9 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_qp_objective", "bik_limits_box", "bik_solve", "bik_solve_ex", "bik_integrate", "bik_check_limits", "bik_step",
            "bik_step_host", "bik_workspace_bytes", "bik_problem_describe", "bik_converge", "bik_track",
            "bik_fk64", "bik_frame_jacobian64", "bik_fk_jac64", "bik_qp_objective64", "bik_limits_box64", "bik_solve64",
-           "bik_integrate64", "bik_check_limits64", "bik_step64", "bik_converge64", "bik_track64", "bik_measure_fma_peak"]
+           "bik_integrate64", "bik_check_limits64", "bik_step64", "bik_converge64", "bik_track64", "bik_measure_fma_peak",
+           "bik_step_weighted", "bik_converge_weighted", "bik_track_weighted", "bik_step_weighted64", "bik_converge_weighted64",
+           "bik_track_weighted64"]
 
 
 class BikError(RuntimeError):
@@ -77,6 +79,11 @@ def load():
     lib.bik_converge64.argtypes = [vp, ci, vp, C.POINTER(BikInputs), cd, cd, ci, cd, cd, ci, vp, vp, vp]
     lib.bik_track64.argtypes = [vp, ci, ci, vp, C.POINTER(BikInputs), vp, cd, cd, ci, cd, cd, ci, vp, vp, vp, vp, vp]
     lib.bik_measure_fma_peak.argtypes = [ci, ci, ci, C.POINTER(cd)]
+    # per-instance task weights: the same arguments with the weights pointer after the inputs
+    for name in ("bik_step", "bik_converge", "bik_track", "bik_step64", "bik_converge64", "bik_track64"):
+        args = getattr(lib, name).argtypes
+        at = args.index(C.POINTER(BikInputs)) + 1
+        getattr(lib, name.replace("64", "") + "_weighted" + ("64" if name.endswith("64") else "")).argtypes = args[:at] + [vp] + args[at:]
     _lib = lib
     return lib
 

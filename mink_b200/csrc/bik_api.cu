@@ -463,8 +463,8 @@ int HostStaging::reserve(const PHeader& h, size_t B, size_t pt_elems) {
 
 // One or more solve_ik steps on device buffers: per step K1 (check_limits + FK + packed task rows + collision rows) and
 // K2 (QP + integrate).  Caller holds p->mu and has reserved the hand-off for `k1d ? 8 : 4`-byte elements.
-static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, double dt, double damping, int nsteps, int integrate,
-                     void* dq, int32_t* status, int io64, bool k1d, cudaStream_t st) {
+static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, const void* weights, double dt, double damping, int nsteps,
+                     int integrate, void* dq, int32_t* status, int io64, bool k1d, cudaStream_t st) {
   // hand-off rows [ws_off, ws_off + B): chunks of one batch may be in flight on different streams (bik_step_host)
   const HandoffSizes n = handoff_sizes(p->h);
   const size_t es = k1d ? 8 : 4;
@@ -479,7 +479,7 @@ static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_in
     K1Args a1;
     memset(&a1, 0, sizeof a1);
     a1.B = B; a1.q = q; a1.ftgt = in->frame_targets; a1.ptgt = in->posture_targets; a1.ctgt = in->com_targets; a1.in64 = io64; a1.pbatched = in->posture_batched;
-    a1.dt = dt; a1.pk = pk; a1.Gc = Gc; a1.hc = hc;
+    a1.dt = dt; a1.pk = pk; a1.Gc = Gc; a1.hc = hc; a1.weights = weights;
     a1.status = status; a1.accumulate = s > 0; a1.tol = 1e-6f;   // Configuration.check_limits(safety_break=False) of solve_ik.py:99
     int rc = phase == 2 ? BIK_OK : bik_launch_k1(p, a1, k1d, st);
     if (rc) return rc;
@@ -495,8 +495,8 @@ static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_in
   return BIK_OK;
 }
 
-static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, double dt, double damping, int nsteps, int integrate, void* dq,
-                       int32_t* status, int f64, void* stream) {
+static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, double dt, double damping, int nsteps,
+                       int integrate, void* dq, int32_t* status, int f64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
   int rc = check_inputs(cp, in, false, f64);
   if (rc) return rc;
@@ -511,15 +511,23 @@ static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* 
   rc = ws_acquire(p, st);
   if (rc) return rc;
   // (status needs no clearing: K1's fused check_limits assigns it on the first step, everything later ORs into it)
-  return ws_release(p, st, step_core(p, B, 0, q, in, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
+  return ws_release(p, st, step_core(p, B, 0, q, in, weights, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
 }
 extern "C" int bik_step(const bik_problem* p, int B, float* q, const bik_inputs* in, float dt, double damping, int nsteps, int integrate, float* dq,
                         int32_t* status, void* stream) {
-  return step_common(p, B, q, in, dt, damping, nsteps, integrate, dq, status, 0, stream);
+  return step_common(p, B, q, in, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
 }
 extern "C" int bik_step64(const bik_problem* p, int B, double* q, const bik_inputs* in, double dt, double damping, int nsteps, int integrate, double* dq,
                           int32_t* status, void* stream) {
-  return step_common(p, B, q, in, dt, damping, nsteps, integrate, dq, status, 1, stream);
+  return step_common(p, B, q, in, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
+}
+extern "C" int bik_step_weighted(const bik_problem* p, int B, float* q, const bik_inputs* in, const void* weights, float dt, double damping, int nsteps,
+                                 int integrate, float* dq, int32_t* status, void* stream) {
+  return step_common(p, B, q, in, weights, dt, damping, nsteps, integrate, dq, status, 0, stream);
+}
+extern "C" int bik_step_weighted64(const bik_problem* p, int B, double* q, const bik_inputs* in, const void* weights, double dt, double damping,
+                                   int nsteps, int integrate, double* dq, int32_t* status, void* stream) {
+  return step_common(p, B, q, in, weights, dt, damping, nsteps, integrate, dq, status, 1, stream);
 }
 
 extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* buf, size_t cap) {
@@ -658,8 +666,8 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   return ws_release(p, st, BIK_OK);
 }
 
-static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, double dt, double damping, int max_iters, double pos_threshold,
-                           double ori_threshold, int check_every, int32_t* iters, int32_t* status, int io64, void* stream) {
+static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, double dt, double damping, int max_iters,
+                           double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
   int rc = check_inputs(cp, in, false, io64);
   if (rc) return rc;
@@ -669,22 +677,33 @@ static int converge_common(const bik_problem* cp, int B, void* q, const bik_inpu
   ConvCall c;
   memset(&c, 0, sizeof c);
   c.B = B; c.T = 1; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
-  c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, io64 != 0); c.io64 = io64 != 0;
+  c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, io64 != 0); c.io64 = io64 != 0; c.weights = weights;
   return converge_run(p, c, check_every, nullptr, static_cast<cudaStream_t>(stream));
 }
 extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
                             float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
+  return converge_common(cp, B, q, in, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
 }
 extern "C" int bik_converge64(const bik_problem* cp, int B, double* q, const bik_inputs* in, double dt, double damping, int max_iters,
                               double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
+  return converge_common(cp, B, q, in, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
+}
+extern "C" int bik_converge_weighted(const bik_problem* cp, int B, float* q, const bik_inputs* in, const void* weights, float dt, double damping,
+                                     int max_iters, float pos_threshold, float ori_threshold, int check_every, int32_t* iters, int32_t* status,
+                                     void* stream) {
+  return converge_common(cp, B, q, in, weights, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
+}
+extern "C" int bik_converge_weighted64(const bik_problem* cp, int B, double* q, const bik_inputs* in, const void* weights, double dt, double damping,
+                                       int max_iters, double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status,
+                                       void* stream) {
+  return converge_common(cp, B, q, in, weights, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
 }
 
 // The examples' outer loop: for each frame of a target sequence, the bik_converge loop, every instance on its own cursor.
 // One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
 // moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
-static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
+static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const void* weights, const int32_t* lengths, double dt,
+                        double damping,
                         int max_iters, double pos_threshold, double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status,
                         int32_t* passes, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
@@ -707,19 +726,31 @@ static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_
   memset(&c, 0, sizeof c);
   c.B = B; c.T = T; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
   c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = true; c.k1d = k1_double(p, damping, io64 != 0);
-  c.io64 = io64 != 0;
+  c.io64 = io64 != 0; c.weights = weights;
   return converge_run(p, c, check_every, passes, st);
 }
 extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
                          int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
                          int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 0,
+  return track_common(cp, B, T, q, in, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 0,
                       stream);
+}
+extern "C" int bik_track_weighted(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights, const int32_t* lengths,
+                                  float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj,
+                                  int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
+                      0, stream);
+}
+extern "C" int bik_track_weighted64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights, const int32_t* lengths,
+                                    double dt, double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
+                                    double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
+                      1, stream);
 }
 extern "C" int bik_track64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
                            int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
                            int32_t* status, int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 1,
+  return track_common(cp, B, T, q, in, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 1,
                       stream);
 }
 
@@ -809,7 +840,7 @@ extern "C" int bik_step_host(const bik_problem* cp, int B, float* q_host, const 
     bik_inputs din = *in;
     din.q = hq + o * nq; din.frame_targets = hft + o * h.F * 7; din.com_targets = hct + o * h.C * 3;
     din.posture_targets = in->posture_batched ? hpt + o * (size_t)h.P * nq : hpt;
-    rc = step_core(p, (int)n, o, hq + o * nq, &din, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
+    rc = step_core(p, (int)n, o, hq + o * nq, &din, nullptr, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
     if (rc) return rc;
     CUDA_OK(cudaEventRecord(hb.hev[2 * ci + 1], s_cmp));
     mark(s_cmp);

@@ -168,12 +168,31 @@ struct K1Args {
   // the thresholds as the fp64 instantiation compares them (the reference tests np.linalg.norm(err[:3]) <= pos_threshold in
   // double); fp32 callers store (double)(float) threshold here, so that the fp64 K1 they may run decides as the fp32 one
   double pos_thr64, ori_thr64;
+  // per-instance task weights of the packed form (null: all ones): [B][K], track mode [B][T][K] (row b*T + cursor[b]), in the
+  // inputs' element type.  Row r of the packed J and e is multiplied by the weight clamped to [0, 1] (NaN: 0), so that K2's
+  // cost_r becomes cost_r * w_r; the errors K1 tests stay unweighted.
+  const void* weights;
 };
 // the thresholds of the convergence test in the instantiation's precision
 template <typename T>
 BIK_HD T k1_pos_thr(const K1Args& a) { if constexpr (sizeof(T) == 8) return a.pos_thr64; else return T(a.pos_thr); }
 template <typename T>
 BIK_HD T k1_ori_thr(const K1Args& a) { if constexpr (sizeof(T) == 8) return a.ori_thr64; else return T(a.ori_thr); }
+// first weight of instance b's rows (a.weights set): the instance's row of [B][K], or in track mode that of its current frame
+template <bool TR>
+BIK_HD long long k1_wbase(const K1Args& a, const PHeader& h, int b) { return (TR ? (long long)b * a.T + a.cursor[b] : (long long)b) * h.K; }
+// weight i of a.weights clamped to [0, 1], NaN to 0
+template <typename T>
+BIK_HD T k1_weight(const K1Args& a, long long i) {
+  const T w = ldin<T>(a.weights, i, a.in64);
+  return w >= T(0) ? (w <= T(1) ? w : T(1)) : T(0);
+}
+template <typename T>
+BIK_HD V3<T> k1_weight3(const K1Args& a, long long i) { return v3<T>(k1_weight<T>(a, i), k1_weight<T>(a, i + 1), k1_weight<T>(a, i + 2)); }
+// the convergence test skips a frame task's position (orientation) error when all three of its weights are 0
+template <typename T>
+BIK_HD bool k1_tested(const K1Args& a, long long i) { return !a.weights || k1_weight<T>(a, i) > T(0) || k1_weight<T>(a, i + 1) > T(0) || k1_weight<T>(a, i + 2) > T(0); }
+template <typename T> BIK_HD V3<T> vmul(V3<T> a, V3<T> b) { return v3<T>(a.x * b.x, a.y * b.y, a.z * b.z); }
 
 // ---- per-warp scratch layout (elements of T) --------------------------------------------------
 BIK_HD int k1_state_stride(const PHeader& h) {  // pose (7) + CoM first moment (3) per node, odd stride
@@ -610,6 +629,13 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         if (v < T(rng[d]) - T(a.tol) || v > T(rng[nv + d]) + T(a.tol)) bad |= 1;
         if (!(v == v)) bad |= 4;
       }
+      if (a.weights) {   // weights outside [0, 1] or NaN: BIK_STATUS_BAD_WEIGHT (they are clamped where they are applied)
+        const long long w0 = k1_wbase<TR>(a, h, inst0 + i);
+        for (int k = lane; k < K; k += W) {
+          const T w = ldin<T>(a.weights, w0 + k, a.in64);
+          if (!(w >= T(0) && w <= T(1))) bad |= 32;
+        }
+      }
       if (bad) {
 #if defined(__CUDA_ARCH__)
         atomicOr(&sflag[i], bad);
@@ -663,6 +689,10 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
       eo[0] = ev.x; eo[1] = ev.y; eo[2] = ev.z; eo[3] = ew.x; eo[4] = ew.y; eo[5] = ew.z;
       if (packed) {   // e rides behind the task's columns
         T* po = pkg + (long long)b * PKS + fr.pk_off + 6 * fr.ncols;
+        if (a.weights) {
+          const long long w0 = k1_wbase<TR>(a, h, b) + fr.row0;
+          ev = vmul(ev, k1_weight3<T>(a, w0)); ew = vmul(ew, k1_weight3<T>(a, w0 + 3));
+        }
         store6<T>(po, ev, ew);
       }
       for (int k = 0; k < 9; ++k) { sc[3 + k] = A1.m[k]; sc[12 + k] = A2.m[k]; }
@@ -725,6 +755,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         q_fr = qmul(qconj(qf), qr);          // rotation of T_rf^-1 = T_fr
         t_fr = qrot_inv(qf, pr - pf);        // translation of T_fr
       }
+      const bool weighted = packed && a.weights;
       for (int c = g; c < fr.ncols; c += G) {
         int ent = cols[fr.col_off + c], d = ent & 0xffff, n = (ent >> 16) & 0x7fff;
         V3<T> jp, jr, tv, tw;
@@ -741,6 +772,10 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
           tw = v3<T>(-bw.x, -bw.y, -bw.z);
         }
         V3<T> top = mmul(A1, tv) + mmul(A2, tw), bot = mmul(A1, tw);
+        if (weighted) {   // (fetched per column: six weights held across the loop make the track-mode kernels spill)
+          const long long w0 = k1_wbase<TR>(a, h, b) + fr.row0;
+          top = vmul(top, k1_weight3<T>(a, w0)); bot = vmul(bot, k1_weight3<T>(a, w0 + 3));
+        }
         if (packed) store6<T>(st + 6 * c, top, bot);
         else {
           st[d] = top.x; st[nv + d] = top.y; st[2 * nv + d] = top.z;
@@ -779,12 +814,19 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         BIK_SYNCWARP();
       }
       if (valid) {
+        const bool weighted = packed && a.weights;
+        V3<T> wc;
+        if (weighted) wc = k1_weight3<T>(a, k1_wbase<TR>(a, h, b) + row0);
         if (g == 0) {
           V3<T> tot = KC<T>::com_fixed(P);
           for (int n = 0; n < h.nnode; ++n) if (P.node(n).parent < 0) tot = tot + ld_v(S + 3 * n);
           T* eo = estage + li * K + row0;  // e = com - target (com_task.py:82); the target was parked here
           eo[0] = tot.x * invM - eo[0]; eo[1] = tot.y * invM - eo[1]; eo[2] = tot.z * invM - eo[2];
-          if (packed) { T* po = pkg + (long long)b * PKS + pk_off + 3 * h.com_ncols; po[0] = eo[0]; po[1] = eo[1]; po[2] = eo[2]; }
+          if (packed) {
+            V3<T> ec = ld_v(eo);
+            if (weighted) ec = vmul(ec, wc);
+            T* po = pkg + (long long)b * PKS + pk_off + 3 * h.com_ncols; po[0] = ec.x; po[1] = ec.y; po[2] = ec.z;
+          }
         }
         T* st = packed ? pkg + (long long)b * PKS + pk_off : stage + li * 3 * nv;
         for (int ci = g; ci < h.com_ncols; ci += G) {
@@ -805,6 +847,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
             }
             col = invM * cross(ax, Sn - Ms * anchor);
           }
+          if (weighted) col = vmul(col, wc);
           if (packed) { st[3 * ci] = col.x; st[3 * ci + 1] = col.y; st[3 * ci + 2] = col.z; }
           else { st[d] = col.x; st[nv + d] = col.y; st[2 * nv + d] = col.z; }
         }
@@ -826,7 +869,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
       for (int f = 0; f < h.F; ++f) {
         const T* eb = estage + lane * K + P.frame(f).row0;
         const T pos = bik_sqrt<T>(eb[0] * eb[0] + eb[1] * eb[1] + eb[2] * eb[2]), ori = bik_sqrt<T>(eb[3] * eb[3] + eb[4] * eb[4] + eb[5] * eb[5]);
-        ok = ok && pos <= k1_pos_thr<T>(a) && ori <= k1_ori_thr<T>(a);
+        const long long w0 = a.weights ? k1_wbase<false>(a, h, inst0 + lane) + P.frame(f).row0 : 0;
+        ok = ok && (pos <= k1_pos_thr<T>(a) || !k1_tested<T>(a, w0)) && (ori <= k1_ori_thr<T>(a) || !k1_tested<T>(a, w0 + 3));
       }
       if (ok) { a.done[inst0 + lane] = 1; a.iters[inst0 + lane] = it; }
       else {
@@ -853,7 +897,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         for (int f = 0; ok && f < h.F; ++f) {
           const T* eb = estage + lane * K + P.frame(f).row0;
           const T pos = bik_sqrt<T>(eb[0] * eb[0] + eb[1] * eb[1] + eb[2] * eb[2]), ori = bik_sqrt<T>(eb[3] * eb[3] + eb[4] * eb[4] + eb[5] * eb[5]);
-          ok = pos <= k1_pos_thr<T>(a) && ori <= k1_ori_thr<T>(a);
+          const long long w0 = a.weights ? k1_wbase<true>(a, h, bi) + P.frame(f).row0 : 0;
+          ok = (pos <= k1_pos_thr<T>(a) || !k1_tested<T>(a, w0)) && (ori <= k1_ori_thr<T>(a) || !k1_tested<T>(a, w0 + 3));
         }
         if (ok || s >= a.conv_max) {
           const int c = a.cursor[bi];

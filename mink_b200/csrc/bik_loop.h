@@ -13,10 +13,11 @@
 namespace bik {
 
 // The arguments of one bik_converge / bik_track call.  io64: fp64 buffers (bik_converge64 / bik_track64).  k1d: K1 runs in
-// fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.
+// fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.  weights: the ..._weighted entry
+// points' per-instance task weights (K1Args::weights), or null.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
-  void* q_traj; int32_t *iters, *status; bool track, k1d, io64;
+  void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights;
 };
 
 // The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
@@ -45,7 +46,7 @@ inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   a.in64 = c.io64; a.dt = c.dt; a.pk = s.pk; a.Gc = s.Gc; a.hc = s.hc;
   a.status = c.track ? s.status : status; a.tol = 1e-6f;
   a.done = s.done; a.iters = c.iters; a.not_done = s.count + 1; a.conv_it = s.count; a.conv_max = c.max_iters;
-  a.pos_thr = (float)c.pos; a.ori_thr = (float)c.ori; a.pos_thr64 = c.pos; a.ori_thr64 = c.ori;
+  a.pos_thr = (float)c.pos; a.ori_thr = (float)c.ori; a.pos_thr64 = c.pos; a.ori_thr64 = c.ori; a.weights = c.weights;
   if (c.track) {
     a.cursor = s.cursor; a.tstep = s.step; a.lengths = c.lengths; a.T = c.T;
     a.q_traj = c.q_traj; a.traj_status = status; a.warm = s.warm;

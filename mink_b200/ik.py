@@ -19,6 +19,10 @@ from .limits import ConfigurationLimit, Limit
 from .tasks import ComTask, FrameTask, PostureTask, Task, problem_for
 
 
+# status bits that fail a solve: BIK_STATUS_QP_MAXITER, _NONFINITE, _QP_INFEASIBLE, _BAD_WEIGHT
+_QP_BITS = 2 | 4 | 8 | 32
+
+
 class Problem(NamedTuple):
     """Stand-in for qpsolvers.Problem: min 1/2 x^T P x + q^T x  s.t.  G x <= h."""
 
@@ -63,6 +67,39 @@ def _lower(configuration: Configuration, tasks: Sequence[Task], limits: Optional
     return prob, kw, limits
 
 
+def _task_weights(tasks: Sequence[Task], weights, q, T: Optional[int] = None):
+    """The [B, K] (track: [B, T, K]) weights buffer of a `weights={task: array}` mapping, rows in the stacked order of J
+    (frame and CoM tasks in list order, 6 and 3 rows), 1 for tasks the mapping leaves out; None for no mapping.
+    Per task: [k] or [B, k]; for a sequence (T given) [k], [T, k] or [B, T, k]."""
+    if not weights:
+        return None
+    import torch
+
+    for task in weights:
+        if not isinstance(task, (FrameTask, ComTask)) or not any(task is t for t in tasks):
+            raise InvalidTarget(f"weights apply to the FrameTask, RelativeFrameTask and ComTask of the task list, not {type(task).__name__}")
+    B = q.shape[0]
+    lead = (B,) if T is None else (B, T)
+    blocks = []
+    for task in tasks:
+        if not isinstance(task, (FrameTask, ComTask)):
+            continue
+        k = 6 if isinstance(task, FrameTask) else 3
+        w = weights.get(task)
+        if w is None:
+            blocks.append(torch.ones(lead + (k,), device=q.device, dtype=q.dtype))
+            continue
+        w = w if isinstance(w, torch.Tensor) else torch.as_tensor(np.array(w, dtype=np.float64))
+        w = w.to(device=q.device, dtype=q.dtype)
+        shapes = [(k,), (B, k)] if T is None else [(k,), (T, k), (B, T, k)]
+        if tuple(w.shape) not in shapes:
+            raise InvalidTarget(f"Expected weights of shape {' or '.join(str(list(s)) for s in shapes)} for {type(task).__name__}, got {list(w.shape)}")
+        if T is not None and w.ndim == 2:
+            w = w.unsqueeze(0)
+        blocks.append(w.expand(lead + (k,)))
+    return torch.cat(blocks, dim=-1).contiguous()
+
+
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
              limits: Optional[Sequence[Limit]] = None) -> Problem:
     """QP of the IK problem (reference solve_ik.py:43-65): P = damping I + sum H_t, q = sum c_t,
@@ -88,8 +125,12 @@ def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, dam
 
 
 def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
-             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, **kwargs):
+             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, **kwargs):
     """Velocity v = dq / dt tangent to the configuration (reference solve_ik.py:68-105).
+
+    `weights` maps a FrameTask / RelativeFrameTask to a [6] or [B, 6] array and a ComTask to a [3] or [B, 3] array of
+    multipliers in [0, 1] of the task's costs (position xyz, orientation xyz): instance b solves with cost * w[b], as if the
+    task's costs had been set to that.  Tasks missing from the mapping keep their costs.
 
     Returns a numpy (nv,) vector for a single configuration, a torch CUDA [B, nv] tensor for a batch.
     Raises NotWithinConfigurationLimits when `safety_break` and some instance is out of limits;
@@ -98,14 +139,15 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     """
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
-    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, **kw)
+    w = _task_weights(tasks, weights, q)
+    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, **kw)
     st = status.cpu().numpy()
     if (st & 1).any():
         if safety_break:
             configuration.check_limits(safety_break=True)
         else:
             configuration.check_limits(safety_break=False)
-    assert not (st & (2 | 4 | 8)).any(), f"QP not solved for {int(((st & 14) != 0).sum())} instance(s) (status bits {np.unique(st & 14)})"
+    assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
     v = dq / float(dt)
     if configuration.batched:
         return v
@@ -114,7 +156,7 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
 
 def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
                 limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-                ori_threshold: float = 1e-4, check_every: int = 1):
+                ori_threshold: float = 1e-4, check_every: int = 1, weights=None):
     """The inner loop the reference's examples wrap around solve_ik (examples/arm_iiwa.py:63-70,
     examples/quadruped_spot.py:89-104), run on the device per instance:
 
@@ -125,14 +167,18 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 
     The configuration is updated in place; returns (iters, converged): steps taken and whether the thresholds were
     met, numpy scalars for a single configuration, [B] numpy arrays for a batch.  A single configuration and a float64
-    batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path."""
+    batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path.
+
+    `weights` as in solve_ik.  A frame task whose three position (orientation) weights are 0 in an instance is left out of
+    that instance's position (orientation) test."""
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
+    w = _task_weights(tasks, weights, q)
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                  ori_threshold=ori_threshold, check_every=check_every, **kw)
+                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, **kw)
     configuration._sync_from_device()
     st = status.cpu().numpy()
-    assert not (st & (2 | 4 | 8)).any(), f"QP not solved for {int(((st & 14) != 0).sum())} instance(s) (status bits {np.unique(st & 14)})"
+    assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
     it, ok = iters.cpu().numpy(), (st & 16) == 0
     if configuration.batched:
         return it, ok
@@ -141,7 +187,7 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1):
+             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -157,6 +203,9 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
 
     Sequences take the configuration's precision: a single configuration and a float64 batch run in fp64 end to end
     (bik_track64), a float32 batch on the fp32 fast path.
+
+    `weights` as in converge_ik, per frame: a task's weights are [6] / [3] (every frame), [T, 6] / [T, 3] (shared by every
+    instance) or [B, T, 6] / [B, T, 3].
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
@@ -196,6 +245,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         return torch.stack(rows, dim=2).contiguous() if rows else None
 
     prob, limits = _problem(configuration, tasks, limits)
+    w = _task_weights(tasks, weights, q, T)
     ln = None
     if lengths is not None:
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
@@ -203,12 +253,12 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
             raise InvalidTarget(f"lengths must have shape ({B},), got {tuple(ln.shape)}")
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), _posture_targets(tasks, flat.nq), stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                          ori_threshold=ori_threshold, check_every=check_every)
+                                          ori_threshold=ori_threshold, check_every=check_every, weights=w)
     configuration._sync_from_device()
     ran = iters >= 0
-    bad = ((status & (2 | 4 | 8)) != 0) & ran
+    bad = ((status & _QP_BITS) != 0) & ran
     n_bad = int(bad.sum())
-    assert n_bad == 0, f"QP not solved for {n_bad} frame(s) (status bits {np.unique((status[bad] & 14).cpu().numpy())})"
+    assert n_bad == 0, f"QP not solved for {n_bad} frame(s) (status bits {np.unique((status[bad] & _QP_BITS).cpu().numpy())})"
     converged = ran & ((status & 16) == 0)
     if configuration.batched:
         return q_traj, iters, converged
