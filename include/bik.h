@@ -128,11 +128,19 @@ typedef struct bik_limit_desc {
 typedef struct bik_inputs {
   const void* q;               /* [B][nq] */
   const void* frame_targets;   /* [B][F][7]  F = number of FRAME + RELATIVE_FRAME tasks, in task-list order */
-  const void* posture_targets; /* [B or 1][P][nq]  P = number of POSTURE tasks */
+  const void* posture_targets; /* layout by posture_batched (below)  P = number of POSTURE tasks */
   const void* com_targets;     /* [B][C][3]  C = number of COM tasks */
-  int32_t posture_batched;     /* 0: one posture target shared by the batch, 1: per instance */
+  int32_t posture_batched;     /* layout of posture_targets, one of BIK_POSTURE_* */
   int32_t f64;                 /* element type of the four buffers: 0 float (fp32 entry points), 1 double (the ...64 ones) */
 } bik_inputs;
+
+/* bik_inputs.posture_batched.  The two sequence forms are accepted by bik_track, bik_track64, bik_track_weighted and
+ * bik_track_weighted64 only: instance b on frame t uses row t of BIK_POSTURE_SEQ_SHARED and row b*T + t of
+ * BIK_POSTURE_SEQ_BATCHED.  Every other entry point rejects them with BIK_ERR_INVALID. */
+#define BIK_POSTURE_SHARED      0  /* [P][nq]: one target shared by the batch */
+#define BIK_POSTURE_BATCHED     1  /* [B][P][nq]: one target per instance (any other value outside 2..3 is read as 1) */
+#define BIK_POSTURE_SEQ_SHARED  2  /* [T][P][nq]: one target per frame, shared by the batch */
+#define BIK_POSTURE_SEQ_BATCHED 3  /* [B][T][P][nq]: one target per instance and frame */
 
 typedef struct bik_dims {
   int32_t nq, nv, nnode;
@@ -238,7 +246,9 @@ int bik_converge(const bik_problem* problem, int B, float* q, const bik_inputs* 
 /* The examples' outer loop (examples/arm_aloha.py:140-169): for each frame t of a target sequence, the bik_converge loop.
  * Each instance moves to its next frame as soon as it is done with the current one; for every instance b the results are
  * those of bik_converge called on frames 0..lengths[b]-1 in turn.  fp32 device buffers, as bik_converge (bik_track64: fp64).
- *   in->frame_targets [B][T][F][7], in->com_targets [B][T][C][3]; posture targets as for bik_converge, the same for every frame
+ *   in->frame_targets [B][T][F][7], in->com_targets [B][T][C][3]; in->posture_targets as for bik_converge (the same for every
+ *   frame), or a sequence: [T][P][nq] with posture_batched = BIK_POSTURE_SEQ_SHARED, [B][T][P][nq] with
+ *   BIK_POSTURE_SEQ_BATCHED (frame t's row then stands where bik_converge's target stands on frame t)
  *   lengths [B] frames per instance, each in 0..T (NULL: all T); q [B][nq] in: start, out: end of each instance's last frame
  *   q_traj [B][T][nq], iters [B][T], status [B][T] (NULL allowed): per frame, as bik_converge returns them; rows past
  *   lengths[b] untouched

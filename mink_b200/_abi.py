@@ -21,6 +21,9 @@ GEOM_PLANE, GEOM_SPHERE, GEOM_CAPSULE, GEOM_BOX = 0, 2, 3, 6
 
 STATUS_OUT_OF_LIMITS, STATUS_QP_MAXITER, STATUS_NONFINITE, STATUS_QP_INFEASIBLE = 1, 2, 4, 8
 
+# BikInputs.posture_batched: [P][nq], [B][P][nq], and the sequences of the bik_track entry points, [T][P][nq] / [B][T][P][nq]
+POSTURE_SHARED, POSTURE_BATCHED, POSTURE_SEQ_SHARED, POSTURE_SEQ_BATCHED = 0, 1, 2, 3
+
 _pd = C.POINTER(C.c_double)
 _pi = C.POINTER(C.c_int32)
 _pf = C.POINTER(C.c_float)

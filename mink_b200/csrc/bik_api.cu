@@ -310,9 +310,13 @@ extern "C" int bik_frame_jacobian64(const bik_model* model, int B, const double*
   return fk_common(model, B, q, frames, nframes, nullptr, nullptr, J, 1, stream);
 }
 
-static int check_inputs(const bik_problem* p, const bik_inputs* in, bool need_q, int f64) {
+// track: a bik_track entry point, the only ones that take a posture target sequence
+static int check_inputs(const bik_problem* p, const bik_inputs* in, bool need_q, int f64, bool track = false) {
   if (!p || !in) return bik_fail(BIK_ERR_INVALID, "null argument");
   const PHeader& h = p->h;
+  if (!track && posture_seq(in))
+    return bik_fail(BIK_ERR_INVALID, "posture_batched = " + std::to_string(in->posture_batched) +
+                                         " (a posture target sequence) is accepted by bik_track, bik_track64 and bik_track_weighted[64] only");
   if ((in->f64 != 0) != (f64 != 0)) return bik_fail(BIK_ERR_INVALID, f64 ? "bik_inputs.f64 must be 1 for the fp64 entry points" : "bik_inputs.f64 must be 0 for the fp32 entry points");
   if (need_q && !in->q) return bik_fail(BIK_ERR_INVALID, "inputs.q is null");
   if (h.F > 0 && !in->frame_targets) return bik_fail(BIK_ERR_INVALID, "No target set for FrameTask");
@@ -443,10 +447,11 @@ int Handoff::reserve(const PHeader& h, size_t B, int elem, unsigned* moves) {
   CUDA_OK(warm.reserve(B * n.warm, moves));
   return BIK_OK;
 }
-int LoopState::reserve(const PHeader& h, size_t B, int elem, unsigned* moves) {
+int LoopState::reserve(const PHeader& h, size_t B, int elem, bool ptseq, unsigned* moves) {
   for (DevBuf* b : {&done, &cursor, &step, &status}) CUDA_OK(b->reserve(sizeof(int32_t) * B, moves));
   CUDA_OK(dq.reserve(elem * B * h.nv, moves));
   CUDA_OK(count.reserve(4 * sizeof(int), moves));
+  if (ptseq) CUDA_OK(ptcur.reserve(elem * B * (size_t)(h.P > 0 ? h.P : 1) * h.nq, moves));
   if (!host) CUDA_OK(cudaMallocHost(&host, 4 * sizeof(int)));
   return BIK_OK;
 }
@@ -558,7 +563,7 @@ static ConvBufs conv_bufs(const bik_problem* p) {
   const Handoff& w = p->hand;
   const LoopState& l = p->loop;
   return ConvBufs{w.pk.ptr, w.Gc.ptr, w.hc.ptr, l.dq.ptr, w.warm.as<signed char>(), l.done.as<int32_t>(), l.cursor.as<int32_t>(), l.step.as<int32_t>(),
-                  l.status.as<int32_t>(), l.count.as<int>()};
+                  l.status.as<int32_t>(), l.count.as<int>(), l.ptcur.ptr};
 }
 // `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
 static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
@@ -642,7 +647,7 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   DeviceGuard g(p->model->device);
   int rc = p->hand.reserve(p->h, c.B, c.k1d ? 8 : 4, &p->moves);
   if (rc) return rc;
-  rc = p->loop.reserve(p->h, c.B, c.io64 ? 8 : 4, &p->moves);   // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
+  rc = p->loop.reserve(p->h, c.B, c.io64 ? 8 : 4, posture_seq(c.in), &p->moves);   // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
   if (rc) return rc;
   rc = ws_acquire(p, st);
   if (rc) return rc;
@@ -707,7 +712,7 @@ static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_
                         int max_iters, double pos_threshold, double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status,
                         int32_t* passes, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, io64);
+  int rc = check_inputs(cp, in, false, io64, true);
   if (rc) return rc;
   if (!q || !q_traj || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (T < 1) return bik_fail(BIK_ERR_INVALID, "T must be at least 1");

@@ -131,9 +131,11 @@ struct LoopState {
   DevBuf dq;                   // [B][nv] K2's dq of the previous pass (its warm start), 4- or 8-byte elements by the caller's precision
   DevBuf cursor, step, status; // [B] each: bik_track's frame cursor, steps taken in that frame, status of the frame in progress
   DevBuf count;                // device: { steps taken so far, unconverged instances, go }
+  DevBuf ptcur;                // [B][P][nq] bik_track's posture targets of each instance's current frame (sequence calls only)
   int* host = nullptr;         // pinned mirror of count
   ConvGraph graph;
-  int reserve(const bik::PHeader& h, size_t B, int elem, unsigned* moves);
+  // elem: bytes of the caller's elements; ptseq: the call has a posture target sequence
+  int reserve(const bik::PHeader& h, size_t B, int elem, bool ptseq, unsigned* moves);
   ~LoopState() { graph.drop(); if (host) cudaFreeHost(host); }
 };
 

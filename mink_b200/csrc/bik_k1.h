@@ -129,7 +129,7 @@ struct K1Args {
   int B;
   const void* q;         // [B][nq]          fp32, or fp64 when in64
   const void* ftgt;      // [B][F][7]
-  const void* ptgt;      // [B or 1][P][nq]
+  const void* ptgt;      // [B or 1][P][nq]; track mode with ptcur set: the sequence, [T][P][nq] (pbatched 2) or [B][T][P][nq] (3)
   const void* ctgt;      // [B][C][3]
   int in64;
   int pbatched;
@@ -172,6 +172,9 @@ struct K1Args {
   // inputs' element type.  Row r of the packed J and e is multiplied by the weight clamped to [0, 1] (NaN: 0), so that K2's
   // cost_r becomes cost_r * w_r; the errors K1 tests stay unweighted.
   const void* weights;
+  // track mode with a posture target sequence (null: none): [B][P][nq] in the inputs' element type.  On the first pass of each
+  // of b's frames K1 copies that frame's posture rows of ptgt into row b; K2 reads this buffer as its per-instance targets.
+  void* ptcur;
 };
 // the thresholds of the convergence test in the instantiation's precision
 template <typename T>
@@ -603,6 +606,23 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         const long long row = (long long)(inst0 + i) * a.T + a.cursor[inst0 + i];
         for (int k = lane; k < FW; k += W) ttile[i * FW + k] = ldin<T>(a.ftgt, row * FW + k, a.in64);
         for (int k = lane; k < CW; k += W) ttile[IPW * FW + i * CW + k] = ldin<T>(a.ctgt, row * CW + k, a.in64);
+      }
+    }
+    if constexpr (TR) {   // first pass of a frame: its posture rows become the instance's row of ptcur, which this pass's K2 reads
+      if (a.ptcur) {
+        const int PW = h.P * nq;
+        for (int i = 0; i < nvalid; ++i) {
+          const int bi = inst0 + i;
+          if (a.tstep[bi] != 0) continue;
+          const long long src = ((a.pbatched == 3 ? (long long)bi * a.T : 0) + a.cursor[bi]) * PW, dst = (long long)bi * PW;
+          // (as for q_traj below: the fp32 instantiations only ever copy fp32 rows)
+          if constexpr (sizeof(T) == 8) {
+            if (a.in64)
+              for (int k = lane; k < PW; k += W) static_cast<double*>(a.ptcur)[dst + k] = static_cast<const double*>(a.ptgt)[src + k];
+          }
+          if (sizeof(T) == 4 || !a.in64)
+            for (int k = lane; k < PW; k += W) static_cast<float*>(a.ptcur)[dst + k] = static_cast<const float*>(a.ptgt)[src + k];
+        }
       }
     }
     if (PK && a.status && lane < IPW) sflag[lane] = 0;

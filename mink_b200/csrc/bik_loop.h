@@ -23,13 +23,19 @@ struct ConvCall {
 // The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
 // the caller's precision.  warm: [B][max(nu,1)] active-set guess.  done: [B] K2 leaves the instance alone.  cursor / step /
 // status: [B] frame each instance is on, steps taken in it (-1: no frames left) and its status (track only).
-// count = { steps taken (converge) or passes run (track), instances left, go }.
+// count = { steps taken (converge) or passes run (track), instances left, go }.  ptcur: [B][P][nq] posture targets of each
+// instance's current frame, in the caller's precision (track with a posture target sequence only, else unused).
 struct ConvBufs {
   void *pk, *Gc, *hc, *dq;
   signed char* warm;
   int32_t *done, *cursor, *step, *status;
   int* count;
+  void* ptcur;
 };
+// bik_inputs.posture_batched names a posture target sequence (bik_track entry points only)
+inline bool posture_seq(const bik_inputs* in) {
+  return in->posture_batched == BIK_POSTURE_SEQ_SHARED || in->posture_batched == BIK_POSTURE_SEQ_BATCHED;
+}
 // Per instance: elements of a pk / Gc / hc row (4 or 8 bytes each, by K1's precision) and bytes of warm.
 struct HandoffSizes { size_t pk, Gc, hc, warm; };
 inline HandoffSizes handoff_sizes(const PHeader& h) {
@@ -50,6 +56,7 @@ inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   if (c.track) {
     a.cursor = s.cursor; a.tstep = s.step; a.lengths = c.lengths; a.T = c.T;
     a.q_traj = c.q_traj; a.traj_status = status; a.warm = s.warm;
+    if (posture_seq(in)) a.ptcur = s.ptcur;
   }
   return a;
 }
@@ -62,6 +69,7 @@ inline K2Args conv_k2_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   a.Gc = s.Gc; a.hc = s.hc; a.gc64 = c.k1d; a.dt = c.dt; a.damping = c.damping; a.dq = s.dq; a.integrate = 1;
   a.status = c.track ? s.status : status;
   a.warm = s.warm; a.skip = s.done; a.gate = s.count + 2;
+  if (posture_seq(in)) { a.ptgt = s.ptcur; a.pbatched = 1; }   // K1 keeps each instance's current frame there
   return a;
 }
 

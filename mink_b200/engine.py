@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._abi import BikDims, BikInputs, ProblemSpec, c_frames
+from ._abi import POSTURE_SEQ_BATCHED, POSTURE_SEQ_SHARED, BikDims, BikInputs, ProblemSpec, c_frames
 from .flatten import FlatModel, Frame
 
 
@@ -276,11 +276,12 @@ class Problem:
 
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-              check_every: int = 1, weights=None):
+              check_every: int = 1, weights=None, posture_seq: bool = False):
         """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
         bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
-        frame_targets [B,T,F,7], com_targets [B,T,C,3]; posture targets as in `converge` (the same for every frame).
+        frame_targets [B,T,F,7], com_targets [B,T,C,3]; posture targets as in `converge` (the same for every frame), or with
+        posture_seq=True a sequence: [T,P,nq] shared by the batch or [B,T,P,nq] per instance.
         q [B,nq] is updated in place to the end of each instance's last frame.
         Returns (q_traj [B,T,nq], iters [B,T], status [B,T], passes): rows past an instance's length hold NaN / -1 / -1;
         passes is a 0-d tensor, the number of passes the device loop ran.
@@ -297,6 +298,11 @@ class Problem:
             if B == 0 or s.shape[0] != B * T or T < 1:
                 raise ValueError(f"target sequences must be [B={B}, T, ...] with the same T >= 1")
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
+        if posture_seq and self.P:
+            n = keep[1 if self.F else 0].numel()   # (_inputs keeps the frame, posture, CoM targets in that order)
+            if n not in (T * self.P * self.nq, B * T * self.P * self.nq):
+                raise ValueError(f"a posture target sequence must be [T={T}, P={self.P}, nq={self.nq}] or [B={B}, T, P, nq]")
+            inp.posture_batched = POSTURE_SEQ_SHARED if n == T * self.P * self.nq else POSTURE_SEQ_BATCHED
         w = self._weights(weights, q, B, T)
         ln = None
         if lengths is not None:

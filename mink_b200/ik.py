@@ -16,7 +16,7 @@ from ._abi import ProblemSpec
 from .configuration import Configuration
 from .exceptions import InvalidTarget
 from .limits import ConfigurationLimit, Limit
-from .tasks import ComTask, FrameTask, PostureTask, Task, problem_for
+from .tasks import ComTask, DampingTask, FrameTask, PostureTask, Task, problem_for
 
 
 # status bits that fail a solve: BIK_STATUS_QP_MAXITER, _NONFINITE, _QP_INFEASIBLE, _BAD_WEIGHT
@@ -204,16 +204,21 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     Sequences take the configuration's precision: a single configuration and a float64 batch run in fp64 end to end
     (bik_track64), a float32 batch on the fp32 fast path.
 
+    A PostureTask takes a [T, nq] or [B, T, nq] sequence of joint-space targets in `targets` as well (a retargeted source
+    motion, say); posture tasks not in `targets` keep their current target on every frame.  A DampingTask's target is qpos0,
+    so it takes no sequence.
+
     `weights` as in converge_ik, per frame: a task's weights are [6] / [3] (every frame), [T, 6] / [T, 3] (shared by every
-    instance) or [B, T, 6] / [B, T, 3].
+    instance) or [B, T, 6] / [B, T, 3].  Posture tasks have no weights.
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
     import torch
 
     for task in targets:
-        if not isinstance(task, (FrameTask, ComTask)):
-            raise InvalidTarget(f"track_ik takes target sequences for FrameTask, RelativeFrameTask and ComTask, not {type(task).__name__}")
+        if not isinstance(task, (FrameTask, ComTask, PostureTask)) or isinstance(task, DampingTask):
+            raise InvalidTarget(f"track_ik takes target sequences for FrameTask, RelativeFrameTask, ComTask and PostureTask, "
+                                f"not {type(task).__name__}")
     flat = configuration.flat
     q = configuration.q_device
     B, dev = q.shape[0], q.device
@@ -222,7 +227,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         t._target()   # TargetNotSet when a task has neither a sequence nor a target
     seqs, T = {}, None
     for task, seq in targets.items():
-        k = 7 if isinstance(task, FrameTask) else 3
+        k = 7 if isinstance(task, FrameTask) else (flat.nq if isinstance(task, PostureTask) else 3)
         if hasattr(seq, "wxyz_xyz"):
             seq = seq.wxyz_xyz
         s = seq if isinstance(seq, torch.Tensor) else torch.as_tensor(np.asarray(seq, dtype=np.float64))
@@ -236,13 +241,24 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         T = s.shape[1]
         seqs[task] = s
     if T is None:
-        raise InvalidTarget("track_ik needs at least one FrameTask / RelativeFrameTask / ComTask target sequence")
+        raise InvalidTarget("track_ik needs at least one FrameTask / RelativeFrameTask / ComTask / PostureTask target sequence")
 
     def stacked(kind, k):
         rows = [seqs[t] if t in seqs else torch.as_tensor(np.asarray(t._target(), dtype=np.float64).reshape(-1, 1, k), device=dev,
                                                           dtype=q.dtype).expand(B, T, k)
                 for t in tasks if isinstance(t, kind)]
         return torch.stack(rows, dim=2).contiguous() if rows else None
+
+    posture, posture_seq = _posture_targets(tasks, flat.nq), False
+    if any(isinstance(t, PostureTask) for t in seqs):
+        # one [1 or B, T, nq] block per posture task (a sequence given without a batch dimension, or a held target shared by
+        # the batch: 1); [T, P, nq] when every block is shared, else [B, T, P, nq]
+        rows = [(seqs[t][:1] if seqs[t].stride(0) == 0 else seqs[t]) if t in seqs else
+                torch.as_tensor(np.asarray(t._target(), dtype=np.float64).reshape(-1, 1, flat.nq), device=dev, dtype=q.dtype).expand(-1, T, -1)
+                for t in tasks if isinstance(t, PostureTask)]
+        lead = max(r.shape[0] for r in rows)
+        posture = torch.stack([r.expand(lead, T, flat.nq) for r in rows], dim=2).contiguous()
+        posture, posture_seq = (posture[0] if lead == 1 else posture), True
 
     prob, limits = _problem(configuration, tasks, limits)
     w = _task_weights(tasks, weights, q, T)
@@ -251,9 +267,9 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
         if ln.shape != (B,):
             raise InvalidTarget(f"lengths must have shape ({B},), got {tuple(ln.shape)}")
-    q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), _posture_targets(tasks, flat.nq), stacked(ComTask, 3), lengths=ln, dt=dt,
+    q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                          ori_threshold=ori_threshold, check_every=check_every, weights=w)
+                                          ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran

@@ -1,6 +1,6 @@
 """Small invocations of every kernel path for compute-sanitizer (memcheck / racecheck): K1 packed and dense (direct + staged),
 K1 fp64, both K2 paths (small-group 32/64-bit masks, general with collision rows), fp64 entry points, bik_converge, bik_track and
-bik_converge64 / bik_track64 (host-polled), bik_step_host.
+bik_converge64 / bik_track64 (host-polled, also with posture target sequences), bik_step_host.
 Ragged batches so that tail tiles run.  Usage:  compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os
 import sys
@@ -48,6 +48,13 @@ for name, env in (("g1", {}), ("g1", {"BIK_K2_PATH": "dense"}), ("g1", {"BIK_USE
     prob.converge(q64, ft, pt, ct, dt=dt, damping=damping, max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2)
     prob.track(q64, fts, pt, seq(ct), lengths=torch.arange(45, device="cuda:0", dtype=torch.int32) % 4, dt=dt, damping=damping,
                max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2)
+    if spec.nposture:   # posture target sequences: per instance (fp32, K1 copies each frame's rows) and shared (fp64)
+        pts = np.broadcast_to(np.asarray(pt, np.float64).reshape(1, 1, spec.nposture, fm.nq), (45, 3, spec.nposture, fm.nq)).copy()
+        pts[:, 1:] += 1e-3 * np.arange(1, 3)[None, :, None, None]
+        prob.track(q, fts, pts, seq(ct), lengths=torch.arange(45, device="cuda:0", dtype=torch.int32) % 4, dt=dt, damping=damping,
+                   max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3, check_every=2, posture_seq=True)
+        prob.track(q64, fts, pts[0], seq(ct), dt=dt, damping=damping, max_iters=4, pos_threshold=2e-3, ori_threshold=2e-3,
+                   check_every=2, posture_seq=True)
     os.environ.pop("BIK_CONVERGE_GRAPH")
     prob.step_host(q0.astype(np.float32), ft, pt, ct, dt=dt, damping=damping, nsteps=1, integrate=True)
     torch.cuda.synchronize()
