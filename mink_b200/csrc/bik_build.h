@@ -455,6 +455,75 @@ inline bool build_image(const HostModel& m, const bik_task_desc* tasks, int ntas
           memcpy(b.w.data() + H.off_geoms64 + GEOM64_WORDS * g, &r, sizeof r);
         }
   }
+  // K2 tables (bik_k2t.h reads them; see PHeader).  Every value is derived from the fp32 records above exactly as the kernel
+  // derived it per tile, and the products are exact or rounded once in double as the kernel rounds them, so K2's results do
+  // not change.  (b.alloc reallocates: the tables above are copied out first.)
+  H.words64 = (int)b.w.size();
+  {
+    const int nt = H.F + H.C, nv = m.nv;
+    const std::vector<int32_t> umap(b.i(H.off_umap), b.i(H.off_umap) + nv);
+    const std::vector<float> posture(b.f(H.off_posture), b.f(H.off_posture) + H.P * (2 + nv));
+    const std::vector<float> cfg(b.f(H.off_cfg), b.f(H.off_cfg) + ncfg * (2 + 2 * nv));
+    const std::vector<float> vmax(b.f(H.off_vmax), b.f(H.off_vmax) + nv);
+    const std::vector<float> com(b.f(H.off_com), b.f(H.off_com) + 8 * H.C);
+    K2Header kh; memset(&kh, 0, sizeof kh);
+    const int khoff = b.alloc(8);
+    kh.tasks = b.alloc(8 * std::max(nt, 1));
+    kh.w = b.alloc(2 * std::max(H.pk_stride, 1));
+    for (int t = 0; t < nt; ++t) {
+      K2TaskRec k; memset(&k, 0, sizeof k);
+      float cost[6], gain;
+      if (t < H.F) {
+        FrameRec fr; memcpy(&fr, b.w.data() + H.off_frames + FRAME_WORDS * t, sizeof fr);
+        k.nr = 6; k.nc = fr.ncols; k.coff = fr.col_off; k.row0 = fr.row0; k.pk_off = fr.pk_off; k.lm = fr.lm;
+        memcpy(cost, fr.cost, sizeof cost); gain = fr.gain;
+      } else {
+        const float* cr = com.data() + 8 * (t - H.F);
+        k.nr = 3; k.nc = H.com_ncols; k.coff = H.com_cols_off; memcpy(&k.row0, cr + 5, 4); memcpy(&k.pk_off, cr + 6, 4); k.lm = cr[4];
+        memcpy(cost, cr, 3 * sizeof(float)); gain = cr[3];
+      }
+      for (int e = 0; e < k.nr * k.nc; ++e) reinterpret_cast<double*>(b.w.data() + kh.w)[k.pk_off + e] = (double)cost[e % k.nr];
+      for (int r = 0; r < k.nr; ++r) reinterpret_cast<double*>(b.w.data() + kh.w)[k.pk_off + k.nr * k.nc + r] = (double)cost[r] * (double)(-gain);
+      // pair schedule of k2t_task_accumulate_nr: where H entry (ia, ib), ib <= ia, lands in the packed triangle
+      k.pairs = b.alloc((k.nc * (k.nc + 1) / 2 + 1) / 2);
+      k.ucol = b.alloc((k.nc + 1) / 2);
+      int16_t* pairs = reinterpret_cast<int16_t*>(b.w.data() + k.pairs);
+      int16_t* ucol = reinterpret_cast<int16_t*>(b.w.data() + k.ucol);
+      for (int ia = 0; ia < k.nc; ++ia) {
+        const int ua = umap[cols[k.coff + ia] & 0xffff];
+        ucol[ia] = (int16_t)ua;
+        for (int ib = 0; ib <= ia; ++ib) {
+          const int ub = umap[cols[k.coff + ib] & 0xffff], hi = std::max(ua, ub), lo = std::min(ua, ub);
+          pairs[ia * (ia + 1) / 2 + ib] = (int16_t)(hi * (hi + 1) / 2 + lo);
+        }
+      }
+      memcpy(b.w.data() + kh.tasks + 8 * t, &k, sizeof k);
+    }
+    kh.dofs = b.alloc(12 * std::max(nv, 1));
+    for (int d = 0; d < nv; ++d) {
+      K2DofRec r; memset(&r, 0, sizeof r);
+      r.qa = m.dof_qadr[d]; r.u = umap[d]; r.vmax = vmax[d];
+      for (int c = 0; c < ncfg; ++c) {
+        const float* p = cfg.data() + c * (2 + 2 * nv);
+        r.cfg[c][0] = p[0]; r.cfg[c][1] = p[2 + d]; r.cfg[c][2] = p[2 + nv + d];
+      }
+      memcpy(b.w.data() + kh.dofs + 12 * d, &r, sizeof r);
+    }
+    // w^2 is exact in double, as is w gain; (gain w) w rounds once, as the kernel's left-to-right product did
+    kh.post = b.alloc(8 * std::max(H.P * nv, 1));
+    for (int p = 0; p < H.P; ++p)
+      for (int d = 0; d < nv; ++d) {
+        const double g = posture[p * (2 + nv)], w = posture[p * (2 + nv) + 2 + d];
+        K2PostRec r = {w * w, (g * w) * w, w * g, 0.0};
+        memcpy(b.w.data() + kh.post + 8 * (p * nv + d), &r, sizeof r);
+      }
+    std::vector<int32_t> quat;
+    for (int n = 0; n < m.nnode; ++n) if (m.node_type[n] == JNT_FREE || m.node_type[n] == JNT_BALL) quat.push_back(n);
+    kh.nquat = (int)quat.size();
+    kh.quat = b.alloc(std::max(kh.nquat, 1));
+    if (!quat.empty()) memcpy(b.i(kh.quat), quat.data(), quat.size() * 4);
+    memcpy(b.w.data() + khoff, &kh, sizeof kh);
+  }
   H.words = (int)b.w.size();
   memcpy(b.w.data() + hoff, &H, sizeof H);
   *image = b.w;

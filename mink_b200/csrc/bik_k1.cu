@@ -62,7 +62,7 @@ template <typename T, int G, bool PK, bool TR>
 static int launch_k1_pk(const bik_problem* p, const K1Args& a, cudaStream_t st) {
   const PHeader& h = p->h;
   constexpr int IPW = 32 / G;
-  const int words = sizeof(T) == 8 ? h.words : h.words32;   // the fp64 side tables only travel with the fp64 instantiation
+  const int words = sizeof(T) == 8 ? h.words64 : h.words32;   // the fp64 side tables only travel with the fp64 instantiation
   int NW = 4;  // warps per CTA: as many as fit next to the image in shared memory
   auto need = [&](int nw) { return (size_t)words * 4 + (size_t)nw * k1_warp_words(h, IPW) * sizeof(T); };
   while (NW > 1 && (int)need(NW) > p->model->max_smem) NW >>= 1;
@@ -100,7 +100,7 @@ template <typename T, int G>
 static int launch_fk(const bik_model* m, const FkArgs& a, cudaStream_t st) {
   const PHeader& h = m->h;
   constexpr int IPW = 32 / G, THREADS = 128, NW = THREADS / 32;
-  const int words = sizeof(T) == 8 ? h.words : h.words32;
+  const int words = sizeof(T) == 8 ? h.words64 : h.words32;
   size_t smem = (size_t)words * 4 + (size_t)NW * fk_warp_words(h, IPW) * sizeof(T);
   int grid = 1;
   long long tiles = ((long long)a.B + IPW - 1) / IPW;

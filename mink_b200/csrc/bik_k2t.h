@@ -114,24 +114,31 @@ BIK_HD int k2t_slot_T_words(const PView& P) { return tri(P.h().nu) + k2t_union_w
 BIK_HD int k2t_slot_bytes(const PView& P, int ts) { return k2t_slot_T_words(P) * ts + 2 * P.h().nu * 4; }
 BIK_HD int k2t_warp_bytes(const PView& P, int ts, int NS) { return (NS * k2t_slot_bytes(P, ts) + 15) & ~15; }   // ts: sizeof(T)
 
+// ---- problem tables built by bik_problem_create (bik_build.h) ------------------------------------------------------------
+BIK_HD const K2Header& k2t_h(const PView& P) { return *reinterpret_cast<const K2Header*>(P.base + P.h().words64); }
+BIK_HD const K2TaskRec& k2t_task(const PView& P, int t) { return reinterpret_cast<const K2TaskRec*>(P.base + k2t_h(P).tasks)[t]; }
+BIK_HD const K2DofRec* k2t_dofs(const PView& P) { return reinterpret_cast<const K2DofRec*>(P.base + k2t_h(P).dofs); }
+BIK_HD const K2PostRec* k2t_post(const PView& P) { return reinterpret_cast<const K2PostRec*>(P.base + k2t_h(P).post); }
+
 // ---- staging (warp-cooperative, W lanes, NS instances) -------------------------------------------------
 // One task's weighted block, column-major like K1's packed record:
 //   tile[i][ia*nr + r] = cost_r J[row0+r][col_ia],   tile[i][nr*nc + r] = cost_r (-gain e[row0+r]).
+// wk: the weights of the task's nr*nc + nr elements (K2Header::w).
 // Source: the packed hand-off (one contiguous run per instance: coalesced without any index arithmetic) or, for bik_solve,
 // the dense rows (gather through the task's column list).  PK: the packed hand-off is known to be there.
 template <typename T, int W, int NS, bool PK = false>
 BIK_HD void k2t_stage_task(T* tile, int S, int lane, int cnt, long long b0, const K2Args& a, int pk64, int dense64, int K, int nv, int pks,
-                           const int32_t* cols, const K2Task& tk) {
+                           const int32_t* cols, const K2TaskRec& tk, const double* wk) {
   const int nj = tk.nr * tk.nc, ne = nj + tk.nr;
   for (int k = lane; k < ne; k += W) {
-    const int ia = k / tk.nr, r = k - ia * tk.nr;
-    const bool isj = k < nj;
-    const T cr = isj ? T(tk.cost[r]) : T(tk.cost[r]) * T(-tk.gain);
+    const T cr = T(wk[k]);
     if (PK || a.pk) {
       const long long o = b0 * pks + tk.pk_off + k;
 #pragma unroll
       for (int i = 0; i < NS; ++i) tile[i * S + k] = i < cnt ? cr * ldin<T>(a.pk, o + (long long)i * pks, pk64) : T(0);
     } else {
+      const int ia = k / tk.nr, r = k - ia * tk.nr;
+      const bool isj = k < nj;
       const void* src = isj ? a.J : a.e;
       const long long o = isj ? b0 * K * nv + (tk.row0 + r) * nv + (cols[ia] & 0xffff) : b0 * K + tk.row0 + r, stride = isj ? (long long)K * nv : K;
 #pragma unroll
@@ -157,9 +164,10 @@ BIK_HD void k2t_stage_rows(T* tile, int S, int off, int lane, int cnt, const voi
 // ---- assembly: (W J)^T (W J) and -(W(-g e))^T W J of one task --------------------------------------------------
 // Whole columns are dealt to the G lanes, heaviest first in serpentine order (column ia pairs with ia + 1 columns, so lane
 // l takes the (l)-th, (2G-1-l)-th, (2G+l)-th ... heaviest).  A lane keeps its column's NR weighted entries in registers and
-// walks the columns ib <= ia: NR loads + NR FMAs per entry of H instead of 2 NR loads and a pair-index decode.
+// walks the columns ib <= ia: NR loads + NR FMAs per entry of H instead of 2 NR loads and a pair-index decode.  Where each entry
+// lands comes from the task's tables (K2TaskRec): ucol[ia] = ua, and pairs[tri(ia) + ib] = its packed-triangle offset.
 template <typename T, int G, int NS, int NR>
-BIK_HD void k2t_task_accumulate_nr(const T* tr, int nc, const int32_t* cols, const int32_t* umap, T* Hp, T* c, int l) {
+BIK_HD void k2t_task_accumulate_nr(const T* tr, int nc, const int16_t* pairs, const int16_t* ucol, T* Hp, T* c, int l) {
   const T* wev = tr + NR * nc;
   for (int rnd = 0;; ++rnd) {
     const int jj = (rnd & 1) ? (rnd + 1) * G - 1 - l : rnd * G + l;
@@ -169,33 +177,34 @@ BIK_HD void k2t_task_accumulate_nr(const T* tr, int nc, const int32_t* cols, con
     T cs = T(0);
 #pragma unroll
     for (int r = 0; r < NR; ++r) { col[r] = tr[ia * NR + r]; cs += wev[r] * col[r]; }
-    const int ua = umap[cols[ia] & 0xffff];
-    c[ua * NS] -= cs;
+    c[ucol[ia] * NS] -= cs;
+    const int16_t* pr = pairs + tri(ia);
     #pragma unroll 1
     for (int ib = 0; ib <= ia; ++ib) {
       const T* cb = tr + ib * NR;
       T s = T(0);
 #pragma unroll
       for (int r = 0; r < NR; ++r) s += col[r] * cb[r];
-      const int ub = umap[cols[ib] & 0xffff];
-      const int hi = ua > ub ? ua : ub, lo = ua > ub ? ub : ua;
-      Hp[(tri(hi) + lo) * NS] += s;
+      Hp[pr[ib] * NS] += s;
     }
   }
 }
 // The CoM task (at most one per problem) is assembled out of line: its unrolled copy would otherwise sit in the kernel
 // beside the frame tasks' one.
 template <typename T, int G, int NS>
-BIK_NOINLINE void k2t_task_accumulate_com(const T* tr, int nc, const int32_t* cols, const int32_t* umap, T* Hp, T* c, int l) {
+BIK_NOINLINE void k2t_task_accumulate_com(const T* tr, int nc, const int16_t* pairs, const int16_t* ucol, T* Hp, T* c, int l) {
   BIK_IN_SHARED(tr); BIK_IN_SHARED(Hp); BIK_IN_SHARED(c);
-  k2t_task_accumulate_nr<T, G, NS, 3>(tr, nc, cols, umap, Hp, c, l);
+  k2t_task_accumulate_nr<T, G, NS, 3>(tr, nc, pairs, ucol, Hp, c, l);
 }
 template <typename T, int G, int NS>
-BIK_HD void k2t_task_accumulate(const T* tr, int nr, int nc, const int32_t* cols, const int32_t* umap, T* Hp, T* c, float lm, T* mu, int l) {
+BIK_HD void k2t_task_accumulate(const PView& P, const T* tr, const K2TaskRec& tk, T* Hp, T* c, T* mu, int l) {
+  const int nr = tk.nr, nc = tk.nc;
   const T* wev = tr + nr * nc;
-  if (lm != 0.f) { T s = T(0); for (int r = 0; r < nr; ++r) s += wev[r] * wev[r]; *mu += T(lm) * s; }
-  if (nr == 6) k2t_task_accumulate_nr<T, G, NS, 6>(tr, nc, cols, umap, Hp, c, l);
-  else k2t_task_accumulate_com<T, G, NS>(tr, nc, cols, umap, Hp, c, l);
+  if (tk.lm != 0.f) { T s = T(0); for (int r = 0; r < nr; ++r) s += wev[r] * wev[r]; *mu += T(tk.lm) * s; }
+  const int16_t* pairs = reinterpret_cast<const int16_t*>(P.base + tk.pairs);
+  const int16_t* ucol = reinterpret_cast<const int16_t*>(P.base + tk.ucol);
+  if (nr == 6) k2t_task_accumulate_nr<T, G, NS, 6>(tr, nc, pairs, ucol, Hp, c, l);
+  else k2t_task_accumulate_com<T, G, NS>(tr, nc, pairs, ucol, Hp, c, l);
 }
 
 // ---- solver pieces: compact run-time loops (the whole pivoting iteration must stay resident in the
@@ -374,23 +383,39 @@ BIK_HD void k2t_schur(T* __restrict__ Hp, const T* __restrict__ Lp, T* __restric
 
 // ---- work that runs once per tile, or for few problems: out of line, so that it does not take instruction-cache room
 // from the solver loops.  Same arithmetic as in line.
-// Levenberg-Marquardt terms of the posture tasks: mu + sum_p lm_p |W_p e_p|^2 (eprow: the staged posture errors).
+// Levenberg-Marquardt terms of the posture tasks: mu + sum_p lm_p |W_p e_p|^2 (eprow: the staged posture errors).  The sum
+// over d stays serial, in dof order: split over the lanes of a group it would be reassociated and change the result's bits.
 template <typename T>
 BIK_NOINLINE T k2t_posture_lm(PView P, const T* eprow, T mu) {
   BIK_IN_SHARED(eprow);
   const PHeader& h = P.h();
   const int nv = h.nv;
+  const K2PostRec* post = k2t_post(P);
   #pragma unroll 1
   for (int p = 0; p < h.P; ++p) {
-    const float* pr = P.f(h.off_posture) + p * (2 + nv);
-    if (pr[1] != 0.f) {
+    const float lm = P.f(h.off_posture)[p * (2 + nv) + 1];
+    if (lm != 0.f) {
       T s = T(0);
       #pragma unroll 1
-      for (int d = 0; d < nv; ++d) { T v = T(pr[2 + d]) * T(pr[0]) * eprow[p * nv + d]; s += v * v; }
-      mu += T(pr[1]) * s;
+      for (int d = 0; d < nv; ++d) { T v = T(post[p * nv + d].wg) * eprow[p * nv + d]; s += v * v; }
+      mu += T(lm) * s;
     }
   }
   return mu;
+}
+// box_dof (bik_k1.h) from the dof's record: the same bounds, combined in the same order
+template <typename T>
+BIK_HD void k2t_box_dof(const K2DofRec& r, int ncfg, int has_vel, T qi, T dt, T* lo, T* hi) {
+  T l = -T(BIK_INF_F), u = T(BIK_INF_F);
+  if (r.qa >= 0) {
+    #pragma unroll 1
+    for (int c = 0; c < ncfg; ++c) {
+      T up = T(r.cfg[c][0]) * (T(r.cfg[c][2]) - qi), dn = T(r.cfg[c][0]) * (qi - T(r.cfg[c][1]));
+      u = bik_min(u, up); l = bik_max(l, -dn);
+    }
+  }
+  if (has_vel) { T vm = dt * T(r.vmax); u = bik_min(u, vm); l = bik_max(l, -vm); }
+  *lo = l; *hi = u;
 }
 // q <- q (+) dq of one free or ball joint (quaternion update)
 template <typename T>
@@ -417,7 +442,6 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   const PHeader& h = P.h();
   const int nv = h.nv, nu = h.nu, K = h.K, nq = h.nq, NP = h.P;
   const int32_t* cols = P.i(h.off_cols);
-  const int32_t* umap = P.i(h.off_umap);
   const int32_t* ucols = P.i(h.off_ucols);
   const int cnt = (a.B - b0) < NS ? (int)(a.B - b0) : NS;
   const int slot = lane / G, l = lane - slot * G;
@@ -442,11 +466,11 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   for (int k = l; k < nu; k += G) c[k * NS] = T(0);
   T mu = T(a.damping);
   for (int t = 0; t < h.F + h.C; ++t) {
-    const K2Task tk = k2_task(P, t);
+    const K2TaskRec& tk = k2t_task(P, t);
     BIK_SYNCWARP();
-    k2t_stage_task<T, W, NS, STEP>(U, St, lane, cnt, b0, a, pk64, dense64, K, nv, h.pk_stride, cols + tk.coff, tk);
+    k2t_stage_task<T, W, NS, STEP>(U, St, lane, cnt, b0, a, pk64, dense64, K, nv, h.pk_stride, cols + tk.coff, tk, P.d(k2t_h(P).w) + tk.pk_off);
     BIK_SYNCWARP();
-    k2t_task_accumulate<T, G, NS>(U + (size_t)slot * St, tk.nr, tk.nc, cols + tk.coff, umap, Hp, c, tk.lm, &mu, l);
+    k2t_task_accumulate<T, G, NS>(P, U + (size_t)slot * St, tk, Hp, c, &mu, l);
   }
   // q and posture errors: stage, then diagonal / linear term / box; decoupled dofs are finished on the spot
   BIK_SYNCWARP();
@@ -469,21 +493,23 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   {
     const T* qrow = U + (size_t)slot * Sq;
     const T* eprow = qrow + nq;
-    const int32_t* dofqadr = P.i(h.off_dofqadr);
     if (NP > 0) mu = k2t_posture_lm<T>(P, eprow, mu);
+    const K2DofRec* dofs = k2t_dofs(P);
+    const K2PostRec* post = k2t_post(P);
     for (int d = l; d < nv; d += G) {
-      const int u = umap[d];
+      const K2DofRec& dr = dofs[d];
+      const int u = dr.u;
+      // hd += w^2 and cd -= ((gain w) w) e per posture task, in task order, as one FMA each: w^2 is exact in double, so
+      // adding the tabled w^2 rounds exactly as fma(w, w, hd) did, and (gain w) w is the product the kernel rounded before
       T hd = mu, cd = T(0);
       #pragma unroll 1
       for (int p = 0; p < NP; ++p) {
-        const float* pr = P.f(h.off_posture) + p * (2 + nv);
-        const T wgt = T(pr[2 + d]);
-        hd += wgt * wgt;
-        cd -= T(pr[0]) * wgt * wgt * eprow[p * nv + d];
+        const K2PostRec& pr = post[p * nv + d];
+        hd += T(pr.w2);
+        cd -= T(pr.gw2) * eprow[p * nv + d];
       }
       T bl, bu;
-      const int qa = dofqadr[d];
-      box_dof<T>(P, d, qa >= 0 ? qrow[qa] : T(0), T(a.dt), &bl, &bu);
+      k2t_box_dof<T>(dr, h.ncfg, h.has_vel, dr.qa >= 0 ? qrow[dr.qa] : T(0), T(a.dt), &bl, &bu);
       if (bl > bu + T(1e-9) * (T(1) + (bu < 0 ? -bu : bu))) st |= 8;   // inconsistent limits: the reference's QP has no solution (solve_ik.py:103)
       if (u >= 0) { Hp[(tri(u) + u) * NS] += hd; c[u * NS] += cd; lo[u * NS] = float(bl); hi[u * NS] = float(bu); }
       else {
@@ -656,7 +682,7 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
         const int i = (int)(((uint32_t)k * mnv) >> 20), d = k - i * nv, qa = dofqadr[d];
         if (qa >= 0 && !(a.skip && a.skip[b0 + i])) qg[(b0 + i) * nq + qa] += dg[(b0 + i) * nv + d];
       }
-      if (live) for (int nn = l; nn < h.nnode; nn += G) { const NodeRec& r = P.node(nn); if (r.type == JNT_FREE || r.type == JNT_BALL) k2t_integrate_quat_node(r, qg + b * nq, dg + b * nv); }
+      if (live) { const K2Header& kh = k2t_h(P); for (int k = l; k < kh.nquat; k += G) k2t_integrate_quat_node(P.node(P.i(kh.quat)[k]), qg + b * nq, dg + b * nv); }
     };
     if (F32IO || !io64) sweep(reinterpret_cast<float*>(const_cast<void*>(a.q)), reinterpret_cast<const float*>(a.dq));   // fp32 buffers: fp32 arithmetic, as bik_integrate
     else sweep(reinterpret_cast<double*>(const_cast<void*>(a.q)), reinterpret_cast<const double*>(a.dq));

@@ -56,6 +56,32 @@ struct GeomRec {  // 16 words
   float pad[4];
 };
 
+// Small-group K2 tables.  One frame / CoM task: its block in the packed record and its column schedule.
+struct K2TaskRec {  // 8 words
+  int32_t nr, nc, coff, row0, pk_off;
+  int32_t pairs;  // word offset of int16 [tri(nc)]: packed-triangle offset tri(ua) + ub of H entry (ia, ib), ib <= ia, at tri(ia) + ib
+  int32_t ucol;   // word offset of int16 [nc]: coupled index ua of each column
+  float lm;
+};
+struct K2DofRec {  // 12 words: what the box of one dof reads (box_dof), and where the dof sits
+  int32_t qa, u;          // qpos address (-1: free / ball dof); coupled index (-1: decoupled)
+  float cfg[MAX_CFG_LIMITS][3];   // per ConfigurationLimit: gain, lower, upper
+  float vmax;
+  int32_t pad[3];
+};
+struct K2PostRec { double w2, gw2, wg, pad; };   // posture task p, dof d: w^2, (gain w) w, w gain (w = cost_eff[d])
+// The small-group K2's tables sit at the end of the image (PHeader::words64), so that no K1 instantiation stages them.  They
+// hold problem constants that the step would otherwise re-derive per tile through chains of dependent loads.
+struct K2Header {  // 8 words; offsets in words from the start of the image
+  int32_t tasks;  // K2TaskRec[F + C]
+  int32_t w;      // double[pk_stride]: the weight of every element of the packed record (cost_r, or cost_r (-gain))
+  int32_t dofs;   // K2DofRec[nv]
+  int32_t post;   // K2PostRec[P][nv]
+  int32_t quat;   // int[nquat]: nodes of the free and ball joints (the quaternion update of integrate)
+  int32_t nquat;
+  int32_t pad[2];
+};
+
 struct PHeader {  // all offsets in 32-bit words from the start of the image
   int32_t words;       // total image size in words (multiple of 4)
   int32_t nq, nv, nnode;
@@ -89,7 +115,8 @@ struct PHeader {  // all offsets in 32-bit words from the start of the image
   int32_t pk_stride;    // elements per instance of the packed K1 -> K2 record (multiple of 4)
   int32_t off_nodes64, off_frames64, off_qpos064, off_comnodes64, off_geoms64;   // fp64 side tables (word offsets, 8-byte aligned)
   int32_t off_com64;    // double { total_mass, fixed[3], coll_gain, coll_dmin, coll_ddet, coll_relax }
-  int32_t reserved[3];
+  int32_t words64;      // words the fp64 kernels of K1 stage; the small-group K2's tables follow, starting with their K2Header
+  int32_t reserved[2];
 };
 static_assert(sizeof(PHeader) % 16 == 0, "header must stay 16-byte aligned");
 
