@@ -49,7 +49,7 @@ typedef enum bik_status {
 #define BIK_STATUS_QP_INFEASIBLE 8u  /* inequality set inconsistent (lower > upper for a dof, or no feasible start): the
                                       * reference's solver returns None there and solve_ik asserts (solve_ik.py:103) */
 #define BIK_STATUS_NOT_CONVERGED 16u /* bik_converge: thresholds not met within max_iters */
-#define BIK_STATUS_BAD_WEIGHT    32u /* ..._weighted entry points: a task weight of the instance is outside [0, 1] or NaN; it was
+#define BIK_STATUS_BAD_WEIGHT    32u /* ..._weighted[_ex] entry points: a task or posture weight of the instance is outside [0, 1] or NaN; it was
                                       * clamped to [0, 1] (NaN to 0) and the step went on with the clamped value */
 
 typedef struct bik_model bik_model;     /* flattened kinematic tree resident on one device */
@@ -325,6 +325,45 @@ int bik_track_weighted64(const bik_problem* problem, int B, int T, double* q, co
                          const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
                          double ori_threshold, int check_every, double* q_traj, int32_t* iters, int32_t* status,
                          int32_t* passes, void* stream);
+
+/* ---- per-instance posture weights --------------------------------------------------------------------------------------
+ * The ..._weighted entry points with one more argument, `posture_weights`, right after `weights`: each instance also scales
+ * the per-dof costs of its own PostureTask and DampingTask, as mink's PostureTask.set_cost would between two solve_ik calls.
+ * A weight of 0 on every dof of a DampingTask drops that task for the instance: one problem serves a batch in which some
+ * instances have the task and others do not.
+ *   posture_weights [B][P][nv] (P = bik_dims.nposture, posture-type tasks in task order as in posture_targets;
+ *           bik_track_weighted_ex: [B][T][P][nv], row b*T + t is used while instance b is on frame t), device memory, float or
+ *           double like the other inputs (bik_inputs.f64).  NULL: exactly what the ..._weighted entry point runs, bit for bit.
+ *           Non-NULL on a problem without posture-type tasks: BIK_ERR_INVALID.
+ *   `weights` as in the ..._weighted entry points, NULL for all ones.
+ *   The cost of posture task p on dof d of instance b is cost[p][d] * w[b][p][d]: it scales the task's diagonal, its part of
+ *   the linear term and its Levenberg-Marquardt term exactly as a cost does.  A weight of exactly 1 gives the unweighted
+ *   arithmetic bit for bit.  Free-joint dofs have no posture rows, so their weights do nothing.  A weight outside [0, 1] is
+ *   clamped to [0, 1], NaN to 0, and the instance (in bik_track: the frame in progress) gets BIK_STATUS_BAD_WEIGHT.  The
+ *   convergence test does not change: it looks at frame errors only.
+ *   Precision of K1 for fp32 callers: posture costs regularise the QP, and the automatic choice of K1's precision counts on
+ *   them.  With posture_weights set it assumes every posture weight may be 0, i.e. it takes the damping alone as the
+ *   regularisation, so a problem that runs K1 in fp32 without posture weights may run it in fp64 with them. */
+int bik_step_weighted_ex(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights,
+                         const void* posture_weights, float dt, double damping, int nsteps, int integrate, float* dq,
+                         int32_t* status, void* stream);
+int bik_converge_weighted_ex(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights,
+                             const void* posture_weights, float dt, double damping, int max_iters, float pos_threshold,
+                             float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_weighted_ex(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights,
+                          const void* posture_weights, const int32_t* lengths, float dt, double damping, int max_iters,
+                          float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters,
+                          int32_t* status, int32_t* passes, void* stream);
+int bik_step_weighted_ex64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights,
+                           const void* posture_weights, double dt, double damping, int nsteps, int integrate, double* dq,
+                           int32_t* status, void* stream);
+int bik_converge_weighted_ex64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights,
+                               const void* posture_weights, double dt, double damping, int max_iters, double pos_threshold,
+                               double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_weighted_ex64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                            const void* posture_weights, const int32_t* lengths, double dt, double damping, int max_iters,
+                            double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
+                            int32_t* status, int32_t* passes, void* stream);
 
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */

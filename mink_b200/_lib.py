@@ -17,7 +17,8 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_fk64", "bik_frame_jacobian64", "bik_fk_jac64", "bik_qp_objective64", "bik_limits_box64", "bik_solve64",
            "bik_integrate64", "bik_check_limits64", "bik_step64", "bik_converge64", "bik_track64", "bik_measure_fma_peak",
            "bik_step_weighted", "bik_converge_weighted", "bik_track_weighted", "bik_step_weighted64", "bik_converge_weighted64",
-           "bik_track_weighted64"]
+           "bik_track_weighted64", "bik_step_weighted_ex", "bik_converge_weighted_ex", "bik_track_weighted_ex",
+           "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64"]
 
 
 class BikError(RuntimeError):
@@ -84,6 +85,8 @@ def load():
         args = getattr(lib, name).argtypes
         at = args.index(C.POINTER(BikInputs)) + 1
         getattr(lib, name.replace("64", "") + "_weighted" + ("64" if name.endswith("64") else "")).argtypes = args[:at] + [vp] + args[at:]
+        # per-instance posture weights: one more pointer after the task weights
+        getattr(lib, name.replace("64", "") + "_weighted_ex" + ("64" if name.endswith("64") else "")).argtypes = args[:at] + [vp, vp] + args[at:]
     _lib = lib
     return lib
 

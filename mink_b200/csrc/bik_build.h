@@ -556,10 +556,12 @@ inline K1Conditioning k1_conditioning(const HostModel& m, const std::vector<uint
   k.min_post2 = std::isfinite(mp) ? mp : 0.0;
   return k;
 }
-// Whether K1 runs in fp64 for an fp32 caller of this problem and damping (BIK_K1_PRECISION aside).
-inline bool k1_auto_double(const PHeader& h, const K1Conditioning& k, double damping) {
+// Whether K1 runs in fp64 for an fp32 caller of this problem and damping (BIK_K1_PRECISION aside).  posture_weighted: the call
+// scales the posture costs per instance (..._weighted_ex with posture weights), possibly down to 0, so only the damping is
+// certain to regularise.
+inline bool k1_auto_double(const PHeader& h, const K1Conditioning& k, double damping, bool posture_weighted = false) {
   if (h.npairs > 0) return true;   // contact points of nearly parallel capsules are ill-conditioned in fp32
-  const double reg = damping + k.min_post2;
+  const double reg = damping + (posture_weighted ? 0.0 : k.min_post2);
   return !(reg > 0) || k.max_cost2 / reg > 1e6;
 }
 

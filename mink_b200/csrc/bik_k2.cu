@@ -5,8 +5,8 @@ using namespace bik;
 
 // W lanes per problem (32 / W problems per warp): 8 or 16 when the augmented factor (coupled dofs + right-hand side) has at most
 // that many rows -- a 6-dof arm with collision rows leaves 26 of 32 lanes idle with a warp per problem.
-template <int W, int SLOTS>
-__global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2Args a) {
+template <int W, int SLOTS, bool PW>
+__device__ __forceinline__ void k2_problems(const uint32_t* __restrict__ gimage, int words, int use_tma, const K2Args& a) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ __align__(8) uint64_t bar;
   if (a.gate && *a.gate == 0) return;
@@ -17,11 +17,22 @@ __global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gi
   const int grp = lane32 / W, lane = lane32 % W;
   char* wsm = reinterpret_cast<char*>(smem + words) + (size_t)(warp * PPW + grp) * k2_warp_bytes(P.h(), sizeof(double));
   for (long long b = (long long)(blockIdx.x * nwarps + warp) * PPW + grp; b < a.B; b += (long long)gridDim.x * nwarps * PPW)
-    k2_warp<double, W, SLOTS>(P, a, (int)b, wsm, lane);
+    k2_warp<double, W, SLOTS, PW>(P, a, (int)b, wsm, lane);
+}
+template <int W, int SLOTS>
+__global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2Args a) {
+  k2_problems<W, SLOTS, false>(gimage, words, use_tma, a);
+}
+// The same with per-instance posture weights (K2PwArgs): the ..._weighted_ex entry points with a posture-weights buffer.
+template <int W, int SLOTS>
+__global__ void __launch_bounds__(256) k2_pw_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2PwArgs a) {
+  k2_problems<W, SLOTS, true>(gimage, words, use_tma, a);
 }
 
-template <int W, int SLOTS>
-static int launch_k2(const bik_problem* p, const K2Args& a, cudaStream_t st) {
+// A: K2Args (k2_kernel) or K2PwArgs (k2_pw_kernel)
+template <int W, int SLOTS, typename A>
+static int launch_k2(const bik_problem* p, const A& a, cudaStream_t st) {
+  constexpr bool PW = std::is_same<A, K2PwArgs>::value;
   const PHeader& h = p->h;
   constexpr int PPW = 32 / W;
   int NW = p->k2_warps;
@@ -30,9 +41,11 @@ static int launch_k2(const bik_problem* p, const K2Args& a, cudaStream_t st) {
   size_t smem = need(NW);
   int grid = 1;
   const long long per_cta = (long long)NW * PPW;
-  int rc = bik_launch_geometry((const void*)k2_kernel<W, SLOTS>, p->model, smem, 32 * NW, ((long long)a.B + per_cta - 1) / per_cta, &grid);
+  const void* kern = PW ? (const void*)k2_pw_kernel<W, SLOTS> : (const void*)k2_kernel<W, SLOTS>;
+  int rc = bik_launch_geometry(kern, p->model, smem, 32 * NW, ((long long)a.B + per_cta - 1) / per_cta, &grid);
   if (rc) return rc;
-  k2_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
+  if constexpr (PW) k2_pw_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
+  else k2_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
@@ -41,7 +54,8 @@ void bik_k2_general_shape(const bik_problem* p, int* lanes, int* slots) {
   *lanes = rows <= 8 ? 8 : (rows <= 16 ? 16 : 32);
   *slots = (rows + *lanes - 1) / *lanes;
 }
-int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) {
+template <typename A>
+static int launch_k2_shape(const bik_problem* p, const A& a, cudaStream_t st) {
   int lanes, slots;
   bik_k2_general_shape(p, &lanes, &slots);
   if (lanes == 8) return launch_k2<8, 1>(p, a, st);
@@ -50,3 +64,5 @@ int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st
   if (slots == 2) return launch_k2<32, 2>(p, a, st);
   return launch_k2<32, 3>(p, a, st);
 }
+int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) { return launch_k2_shape(p, a, st); }
+int bik_launch_k2_general(const bik_problem* p, const K2PwArgs& a, cudaStream_t st) { return launch_k2_shape(p, a, st); }

@@ -78,6 +78,16 @@ struct K2Args {
   const int32_t* skip; // [B] or null: instances marked here are neither solved nor integrated (bik_converge: already converged)
   const int* gate;     // device flag or null: the whole launch is a no-op when it reads 0 (bik_converge's last pass through the graph body)
 };
+// The arguments of the posture-weighted instantiations (PW; the ..._weighted_ex entry points): K2Args and the per-instance
+// posture weights.  A struct of its own, so that the kernels without posture weights keep their parameter block as it is.
+struct K2PwArgs : K2Args {
+  // [B][P][nv], element type follows io64.  Track mode: [B][T][P][nv], row b*pw_T + pw_cursor[b] -- K1 ends a frame in the pass
+  // that moves the cursor and leaves the instance out of that pass's K2, so whenever K2 solves b the cursor names the frame
+  // being solved.
+  const void* pw;
+  const int32_t* pw_cursor;   // [B] or null (step / converge)
+  int pw_T;
+};
 
 enum { K2_MAX_GEN = 24 };  // general (collision) rows that may be active at once; more than that sets BIK_STATUS_QP_MAXITER
 
@@ -197,6 +207,22 @@ template <typename T> BIK_HD K2Ws<T> k2_carve(const PHeader& h, void* mem) {
 
 template <typename T> BIK_HD T Hsym(const T* Hp, int i, int j) { return i >= j ? Hp[tri(i) + j] : Hp[tri(j) + i]; }
 
+// ---- per-instance posture weights (K2PwArgs) ---------------------------------------------------------------------------
+// instance b's posture weights: its [P][nv] block, or in track mode that of its current frame.  `a` is the K2PwArgs a PW
+// instantiation was launched with.
+BIK_HD const void* k2_pw_row(const K2Args& a, const PHeader& h, long long b, int is64) {
+  const K2PwArgs& pa = static_cast<const K2PwArgs&>(a);
+  const long long r = pa.pw_cursor ? b * pa.pw_T + pa.pw_cursor[b] : b;
+  return reinterpret_cast<const char*>(pa.pw) + r * h.P * h.nv * (is64 ? 8 : 4);
+}
+// weight i of pw clamped to [0, 1], NaN to 0; a weight that needed it sets BIK_STATUS_BAD_WEIGHT (32) in *st
+template <typename T>
+BIK_HD T k2_pw(const void* pw, long long i, int is64, int* st) {
+  const T w = ldin<T>(pw, i, is64);
+  if (!(w >= T(0) && w <= T(1))) *st |= 32;
+  return w >= T(0) ? (w <= T(1) ? w : T(1)) : T(0);
+}
+
 // One task of the stacked objective: rows, non-zero columns and where its block sits in the packed record.
 struct K2Task { int row0, nr, nc, coff, pk_off; const float* cost; float gain, lm; };
 BIK_HD K2Task k2_task(const PView& P, int t) {
@@ -212,7 +238,9 @@ BIK_HD K2Task k2_task(const PView& P, int t) {
 }
 
 // ---- assembly ------------------------------------------------------------------------------
-template <typename T, int W>
+// PW (compile time): per-instance posture weights (K2PwArgs, which `a` then is): the cost of posture task p on dof d is
+// cost_eff[d] * w.
+template <typename T, int W, bool PW = false>
 BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int lane) {
   const PHeader& h = P.h();
   const int n = h.nv, nu = h.nu, K = h.K, nq = h.nq;
@@ -278,11 +306,18 @@ BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int l
     const long long t0 = ((long long)(a.pbatched ? b : 0) * h.P + p) * nq;
     return posture_err_dof<T>(P, d, [&](int i) { return ldin<T>(a.ptgt, t0 + i, a.io64); }, qv);
   };
+  const void* pw = nullptr;
+  if constexpr (PW) pw = k2_pw_row(a, h, b, a.io64);
   for (int p = 0; p < h.P; ++p) {
     const float* pr = P.f(h.off_posture) + p * (2 + n);
     if (pr[1] != 0.f) {
       T s = T(0);
-      for (int d = lane; d < n; d += W) { T v = T(pr[2 + d]) * T(pr[0]) * eperr(p, d); s += v * v; }
+      for (int d = lane; d < n; d += W) {
+        T wgt = T(pr[2 + d]);
+        if constexpr (PW) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
+        T v = wgt * T(pr[0]) * eperr(p, d);
+        s += v * v;
+      }
       s = warp_sum_t<W, T>(s);
       mu += T(pr[1]) * s;
     }
@@ -295,6 +330,7 @@ BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int l
     for (int p = 0; p < h.P; ++p) {
       const float* pr = P.f(h.off_posture) + p * (2 + n);
       T wgt = T(pr[2 + d]);
+      if constexpr (PW) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
       hd += wgt * wgt;                                  // (W J)^T (W J), J = -I
       if (wgt != T(0)) cd -= T(pr[0]) * wgt * wgt * eperr(p, d);  // -(W(-g e))^T W (-I)
     }
@@ -717,14 +753,14 @@ BIK_HD int k2_solve(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int lane
 }
 
 // One instance per warp: assemble, optionally dump (H, c) / (lo, hi), solve, write dq, optionally integrate q.
-template <typename T, int W, int SLOTS>
+template <typename T, int W, int SLOTS, bool PW = false>
 BIK_HD void k2_warp(const PView& P, const K2Args& a, int b, void* wsm, int lane) {
   const PHeader& h = P.h();
   const int n = h.nv, nu = h.nu, nq = h.nq;
   const int32_t* umap = P.i(h.off_umap);
   if (a.skip && a.skip[b]) return;
   K2Ws<T> w = k2_carve<T>(h, wsm);
-  int st = k2_assemble<T, W>(P, a, b, w, lane);
+  int st = k2_assemble<T, W, PW>(P, a, b, w, lane);
   if (a.skip_objective) return;
   if (a.Hout) {
     for (int k = lane; k < n * n; k += W) {
@@ -743,7 +779,9 @@ BIK_HD void k2_warp(const PView& P, const K2Args& a, int b, void* wsm, int lane)
     w.xfull[d] = v;
     stout<T>(a.dq, (long long)b * n + d, a.io64, v);
   }
+  const int bw = st & 32;   // BIK_STATUS_BAD_WEIGHT of a posture weight this lane read (PW only)
   st = warp_max_i<W>(st & 2) | warp_max_i<W>(st & 4) | warp_max_i<W>(st & 8);
+  if constexpr (PW) st |= warp_max_i<W>(bw);
   if (lane == 0) {
     if (a.status) a.status[b] |= st;
     if (a.iters) a.iters[b] = iters;

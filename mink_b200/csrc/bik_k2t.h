@@ -403,6 +403,46 @@ BIK_NOINLINE T k2t_posture_lm(PView P, const T* eprow, T mu) {
   }
   return mu;
 }
+// The same with per-instance posture weights (K2PwArgs): the tabled w gain of (p, d) is scaled by the instance's weight
+// before it enters the product.  pw: the instance's [P][nv] weights (element type by pw64), or null for a slot without an
+// instance (its result is not used).  Weights are clamped as k2_pw does; the status bit is left to the diagonal loop, which
+// reads every weight of the instance too.
+template <typename T>
+BIK_NOINLINE T k2t_posture_lm_pw(PView P, const T* eprow, T mu, const void* pw, int pw64) {
+  BIK_IN_SHARED(eprow);
+  const PHeader& h = P.h();
+  const int nv = h.nv;
+  const K2PostRec* post = k2t_post(P);
+  int st = 0;
+  #pragma unroll 1
+  for (int p = 0; p < h.P; ++p) {
+    const float lm = P.f(h.off_posture)[p * (2 + nv) + 1];
+    if (lm != 0.f) {
+      T s = T(0);
+      #pragma unroll 1
+      for (int d = 0; d < nv; ++d) {
+        const T om = pw ? k2_pw<T>(pw, p * nv + d, pw64, &st) : T(1);
+        T v = (T(post[p * nv + d].wg) * om) * eprow[p * nv + d];
+        s += v * v;
+      }
+      mu += T(lm) * s;
+    }
+  }
+  return mu;
+}
+// Start moving `bytes` bytes at p into L2 (the G lanes of a group take a 32-byte sector each in turn); a no-op on the host.
+// The posture weights of a tile's instances are fetched this way when the tile starts: the diagonal loop reads them one
+// dependent load per dof, on the tile's serial chain, long after the task assembly has hidden the trip to memory.
+template <int G>
+BIK_HD void k2t_prefetch_l2(const void* p, int bytes, int l) {
+#if defined(__CUDA_ARCH__)
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), a0 = a & ~uintptr_t(31);
+  #pragma unroll 1
+  for (uintptr_t o = a0 + 32u * l; o < a + bytes; o += 32u * G) asm volatile("prefetch.global.L2 [%0];" ::"l"(o));
+#else
+  (void)p; (void)bytes; (void)l;
+#endif
+}
 // box_dof (bik_k1.h) from the dof's record: the same bounds, combined in the same order
 template <typename T>
 BIK_HD void k2t_box_dof(const K2DofRec& r, int ncfg, int has_vel, T qi, T dt, T* lo, T* hi) {
@@ -433,7 +473,10 @@ BIK_NOINLINE void k2t_store_warm(signed char* wm, int nu, M lom, M upm) {
 // element types follow the run-time flags of K2Args.
 // STEP (compile time, with F32IO): the form bik_step / bik_step_host / bik_converge launch -- packed task rows (a.pk set,
 // a.ep null).  Only the packed staging is compiled in: no dense-row staging, no staging of dense posture errors.
-template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false>
+// PW (compile time): per-instance posture weights (K2PwArgs, which `a` then is; the ..._weighted_ex entry points): the tabled coefficients of
+// posture task p on dof d are scaled by the instance's weight (w^2 and (gain w) w by its square) before they enter the same
+// sums in the same order, so a weight of 1 gives the bits of the unweighted instantiation.
+template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false, bool PW = false>
 BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* wsm, int lane, int St = 0, int uw = 0) {
   static_assert(!STEP || F32IO, "the step instantiation reads fp32 buffers");
   if (St == 0) { St = k2t_task_tile_words(P); uw = k2t_union_words(P); }   // callers that loop over tiles pass them in
@@ -448,6 +491,14 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   const long long b = b0 + slot;
   const bool live = slot < cnt && !(a.skip && a.skip[b]);
   if (a.skip && !BIK_WARP_ANY(live)) return;   // bik_converge: every instance of this tile has converged
+  // PW: this instance's posture weights (null for a slot without a live instance: its results are not stored)
+  const void* pw = nullptr;
+  if constexpr (PW) {
+    if (live && NP > 0) {
+      pw = k2_pw_row(a, h, b, io64);
+      k2t_prefetch_l2<G>(pw, NP * nv * (io64 ? 8 : 4), l);
+    }
+  }
   T* const Tb = reinterpret_cast<T*>(wsm);
   T* const Hp = Tb + slot;
   T* const U = Tb + (size_t)tri(nu) * NS;   // warp-wide base of the union region
@@ -493,7 +544,8 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   {
     const T* qrow = U + (size_t)slot * Sq;
     const T* eprow = qrow + nq;
-    if (NP > 0) mu = k2t_posture_lm<T>(P, eprow, mu);
+    if constexpr (PW) { if (NP > 0) mu = k2t_posture_lm_pw<T>(P, eprow, mu, pw, io64); }
+    else { if (NP > 0) mu = k2t_posture_lm<T>(P, eprow, mu); }
     const K2DofRec* dofs = k2t_dofs(P);
     const K2PostRec* post = k2t_post(P);
     for (int d = l; d < nv; d += G) {
@@ -505,8 +557,14 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
       #pragma unroll 1
       for (int p = 0; p < NP; ++p) {
         const K2PostRec& pr = post[p * nv + d];
-        hd += T(pr.w2);
-        cd -= T(pr.gw2) * eprow[p * nv + d];
+        if constexpr (PW) {
+          const T om = pw ? k2_pw<T>(pw, p * nv + d, io64, &st) : T(1), om2 = om * om;
+          hd += T(pr.w2) * om2;
+          cd -= (T(pr.gw2) * om2) * eprow[p * nv + d];
+        } else {
+          hd += T(pr.w2);
+          cd -= T(pr.gw2) * eprow[p * nv + d];
+        }
       }
       T bl, bu;
       k2t_box_dof<T>(dr, h.ncfg, h.has_vel, dr.qa >= 0 ? qrow[dr.qa] : T(0), T(a.dt), &bl, &bu);

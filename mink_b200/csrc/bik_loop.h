@@ -14,10 +14,11 @@ namespace bik {
 
 // The arguments of one bik_converge / bik_track call.  io64: fp64 buffers (bik_converge64 / bik_track64).  k1d: K1 runs in
 // fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.  weights: the ..._weighted entry
-// points' per-instance task weights (K1Args::weights), or null.
+// points' per-instance task weights (K1Args::weights), or null.  posture_weights: the ..._weighted_ex entry points' per-instance
+// posture weights (K2PwArgs), or null.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
-  void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights;
+  void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights;
 };
 
 // The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
@@ -70,6 +71,15 @@ inline K2Args conv_k2_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   a.status = c.track ? s.status : status;
   a.warm = s.warm; a.skip = s.done; a.gate = s.count + 2;
   if (posture_seq(in)) { a.ptgt = s.ptcur; a.pbatched = 1; }   // K1 keeps each instance's current frame there
+  return a;
+}
+// The same for the posture-weighted K2 (c.posture_weights set).  Track mode reads the row of each instance's current frame.
+inline K2PwArgs conv_k2_pw_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  K2PwArgs a;
+  memset(&a, 0, sizeof a);
+  static_cast<K2Args&>(a) = conv_k2_args(c, s, status);
+  a.pw = c.posture_weights;
+  if (c.track) { a.pw_cursor = s.cursor; a.pw_T = c.T; }
   return a;
 }
 

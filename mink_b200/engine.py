@@ -179,6 +179,17 @@ class Problem:
             raise ValueError(f"weights must have shape {tuple(lead) + (self.K,)} (rows of the stacked task Jacobian), got {tuple(w.shape)}")
         return w
 
+    def _posture_weights(self, posture_weights, q: torch.Tensor, *lead):
+        """Per-instance posture weights as a contiguous [*lead, P, nv] CUDA tensor of q's dtype (None stays None)."""
+        if posture_weights is None:
+            return None
+        if not self.P:
+            raise ValueError("posture_weights given for a problem without a PostureTask or DampingTask")
+        w = self.model._dev(posture_weights, dtype=q.dtype)
+        if tuple(w.shape) != tuple(lead) + (self.P, self.nv):
+            raise ValueError(f"posture_weights must have shape {tuple(lead) + (self.P, self.nv)} (posture-type tasks x dofs), got {tuple(w.shape)}")
+        return w
+
     def fk_jac(self, q, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2):
         inp, keep, B, q = self._inputs(q, frame_targets, posture_targets, com_targets)
         dev, dt_ = q.device, q.dtype
@@ -228,21 +239,27 @@ class Problem:
 
     def step(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
              damping: float = 1e-12, nsteps: int = 1, integrate: bool = False, dq: Optional[torch.Tensor] = None,
-             status: Optional[torch.Tensor] = None, weights=None):
+             status: Optional[torch.Tensor] = None, weights=None, posture_weights=None):
         """solve_ik (x nsteps, optionally integrating q in place).  q: [B,nq] fp32 or fp64 CUDA tensor.
         weights: [B, K] per-instance multipliers in [0, 1] of the frame / CoM task costs, rows in the stacked order of J
-        (bik_step_weighted); None: the problem's costs."""
+        (bik_step_weighted); None: the problem's costs.
+        posture_weights: [B, P, nv] per-instance multipliers in [0, 1] of the PostureTask / DampingTask dof costs, tasks in the
+        order of the posture targets (bik_step_weighted_ex); None: the problem's costs."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
         w = self._weights(weights, q, B)
+        pw = self._posture_weights(posture_weights, q, B)
         if dq is None:
             dq = torch.empty((B, self.nv), device=q.device, dtype=q.dtype)
         if status is None:
             status = torch.empty(B, device=q.device, dtype=torch.int32)
         assert dq.dtype == q.dtype
         args = (float(dt), float(damping), int(nsteps), int(bool(integrate)), dq.data_ptr(), status.data_ptr(), _stream())
-        if w is None:
+        if pw is not None:
+            fn = self.lib.bik_step_weighted_ex64 if _is64(q) else self.lib.bik_step_weighted_ex
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), pw.data_ptr(), *args))
+        elif w is None:
             fn = self.lib.bik_step64 if _is64(q) else self.lib.bik_step
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), *args))
         else:
@@ -252,21 +269,26 @@ class Problem:
 
     def converge(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
                  damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-                 check_every: int = 1, weights=None):
+                 check_every: int = 1, weights=None, posture_weights=None):
         """solve_ik + integrate until every frame task is within the thresholds or max_iters steps were taken, per instance
         (the inner loop of the reference's examples; bik_converge for a float32 q, bik_converge64 for a float64 q, the
         targets in q's dtype).  q is updated in place.  weights: [B, K] as in `step` (bik_converge_weighted); a frame task
         whose three position (orientation) weights are 0 is left out of the position (orientation) test.
+        posture_weights: [B, P, nv] as in `step` (bik_converge_weighted_ex).
         Returns (iters [B], status [B])."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
         w = self._weights(weights, q, B)
+        pw = self._posture_weights(posture_weights, q, B)
         iters = torch.zeros(B, device=q.device, dtype=torch.int32)
         status = torch.zeros(B, device=q.device, dtype=torch.int32)
         args = (float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every), iters.data_ptr(),
                 status.data_ptr(), _stream())
-        if w is None:
+        if pw is not None:
+            fn = self.lib.bik_converge_weighted_ex64 if _is64(q) else self.lib.bik_converge_weighted_ex
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), pw.data_ptr(), *args))
+        elif w is None:
             fn = self.lib.bik_converge64 if _is64(q) else self.lib.bik_converge
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), *args))
         else:
@@ -276,7 +298,7 @@ class Problem:
 
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-              check_every: int = 1, weights=None, posture_seq: bool = False):
+              check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None):
         """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
         bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
@@ -285,7 +307,8 @@ class Problem:
         q [B,nq] is updated in place to the end of each instance's last frame.
         Returns (q_traj [B,T,nq], iters [B,T], status [B,T], passes): rows past an instance's length hold NaN / -1 / -1;
         passes is a 0-d tensor, the number of passes the device loop ran.
-        weights: [B, T, K] per-frame task weights as in `converge` (bik_track_weighted), or None."""
+        weights: [B, T, K] per-frame task weights as in `converge` (bik_track_weighted), or None.
+        posture_weights: [B, T, P, nv] per-frame posture weights as in `converge` (bik_track_weighted_ex), or None."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         m = self.model
         B = q.shape[0]
@@ -304,6 +327,7 @@ class Problem:
                 raise ValueError(f"a posture target sequence must be [T={T}, P={self.P}, nq={self.nq}] or [B={B}, T, P, nq]")
             inp.posture_batched = POSTURE_SEQ_SHARED if n == T * self.P * self.nq else POSTURE_SEQ_BATCHED
         w = self._weights(weights, q, B, T)
+        pw = self._posture_weights(posture_weights, q, B, T)
         ln = None
         if lengths is not None:
             ln = m._dev(lengths, torch.int32).reshape(-1)
@@ -315,7 +339,10 @@ class Problem:
         passes = torch.zeros(1, device=q.device, dtype=torch.int32)
         args = (_ptr(ln), float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every),
                 q_traj.data_ptr(), iters.data_ptr(), status.data_ptr(), passes.data_ptr(), _stream())
-        if w is None:
+        if pw is not None:
+            fn = self.lib.bik_track_weighted_ex64 if _is64(q) else self.lib.bik_track_weighted_ex
+            _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), pw.data_ptr(), *args))
+        elif w is None:
             fn = self.lib.bik_track64 if _is64(q) else self.lib.bik_track
             _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), *args))
         else:

@@ -100,6 +100,41 @@ def _task_weights(tasks: Sequence[Task], weights, q, T: Optional[int] = None):
     return torch.cat(blocks, dim=-1).contiguous()
 
 
+def _posture_weights(tasks: Sequence[Task], posture_weights, q, nv: int, T: Optional[int] = None):
+    """The [B, P, nv] (track: [B, T, P, nv]) posture-weights buffer of a `posture_weights={task: w}` mapping, P the PostureTask /
+    DampingTask of the task list in list order, 1 for those the mapping leaves out; None for no mapping.
+    Per task: a float, [nv] or [B, nv]; for a sequence (T given) also [T, nv] or [B, T, nv]."""
+    if not posture_weights:
+        return None
+    import torch
+
+    for task in posture_weights:
+        if not isinstance(task, PostureTask) or not any(task is t for t in tasks):
+            raise InvalidTarget(f"posture_weights apply to the PostureTask and DampingTask of the task list, not {type(task).__name__}")
+    B = q.shape[0]
+    lead = (B,) if T is None else (B, T)
+    blocks = []
+    for task in tasks:
+        if not isinstance(task, PostureTask):
+            continue
+        w = posture_weights.get(task)
+        if w is None:
+            blocks.append(torch.ones(lead + (nv,), device=q.device, dtype=q.dtype))
+            continue
+        w = w if isinstance(w, torch.Tensor) else torch.as_tensor(np.array(w, dtype=np.float64))
+        w = w.to(device=q.device, dtype=q.dtype)
+        shapes = [(), (nv,), (B, nv)] if T is None else [(), (nv,), (B, nv), (T, nv), (B, T, nv)]
+        if tuple(w.shape) not in shapes:
+            raise InvalidTarget(f"Expected posture weights of shape {' or '.join(str(list(s)) for s in shapes)} for {type(task).__name__}, "
+                                f"got {list(w.shape)}")
+        if T is not None and w.ndim == 2:
+            if B == T and B > 1:
+                raise InvalidTarget(f"posture weights of shape {list(w.shape)} could be [B, nv] or [T, nv] (B = T = {B}): pass [B, T, nv]")
+            w = w.unsqueeze(1) if w.shape[0] == B else w.unsqueeze(0)
+        blocks.append(w.expand(lead + (nv,)))
+    return torch.stack(blocks, dim=-2).contiguous()
+
+
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
              limits: Optional[Sequence[Limit]] = None) -> Problem:
     """QP of the IK problem (reference solve_ik.py:43-65): P = damping I + sum H_t, q = sum c_t,
@@ -125,12 +160,16 @@ def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, dam
 
 
 def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
-             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, **kwargs):
+             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, posture_weights=None, **kwargs):
     """Velocity v = dq / dt tangent to the configuration (reference solve_ik.py:68-105).
 
     `weights` maps a FrameTask / RelativeFrameTask to a [6] or [B, 6] array and a ComTask to a [3] or [B, 3] array of
     multipliers in [0, 1] of the task's costs (position xyz, orientation xyz): instance b solves with cost * w[b], as if the
     task's costs had been set to that.  Tasks missing from the mapping keep their costs.
+
+    `posture_weights` maps a PostureTask / DampingTask to a float, an [nv] or a [B, nv] array of multipliers in [0, 1] of the
+    task's per-dof costs: instance b solves as if the task's cost had been set to cost * w[b] (PostureTask.set_cost).  A
+    weight of 0 on every dof of a DampingTask solves that instance as if the task were not in the list.
 
     Returns a numpy (nv,) vector for a single configuration, a torch CUDA [B, nv] tensor for a batch.
     Raises NotWithinConfigurationLimits when `safety_break` and some instance is out of limits;
@@ -140,7 +179,8 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
-    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, **kw)
+    pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
+    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, **kw)
     st = status.cpu().numpy()
     if (st & 1).any():
         if safety_break:
@@ -156,7 +196,7 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
 
 def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
                 limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-                ori_threshold: float = 1e-4, check_every: int = 1, weights=None):
+                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None):
     """The inner loop the reference's examples wrap around solve_ik (examples/arm_iiwa.py:63-70,
     examples/quadruped_spot.py:89-104), run on the device per instance:
 
@@ -170,12 +210,13 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path.
 
     `weights` as in solve_ik.  A frame task whose three position (orientation) weights are 0 in an instance is left out of
-    that instance's position (orientation) test."""
+    that instance's position (orientation) test.  `posture_weights` as in solve_ik."""
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
+    pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, **kw)
+                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, **kw)
     configuration._sync_from_device()
     st = status.cpu().numpy()
     assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
@@ -187,7 +228,7 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None):
+             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -209,7 +250,10 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     so it takes no sequence.
 
     `weights` as in converge_ik, per frame: a task's weights are [6] / [3] (every frame), [T, 6] / [T, 3] (shared by every
-    instance) or [B, T, 6] / [B, T, 3].  Posture tasks have no weights.
+    instance) or [B, T, 6] / [B, T, 3].  Posture tasks have no `weights`.
+
+    `posture_weights` as in converge_ik, per frame: a PostureTask's or DampingTask's weights are a float, [nv] or [B, nv]
+    (every frame), [T, nv] (shared by every instance) or [B, T, nv] (a 2-D array must then not leave B = T ambiguous).
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
@@ -262,6 +306,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
 
     prob, limits = _problem(configuration, tasks, limits)
     w = _task_weights(tasks, weights, q, T)
+    pw = _posture_weights(tasks, posture_weights, q, flat.nv, T)
     ln = None
     if lengths is not None:
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
@@ -269,7 +314,8 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
             raise InvalidTarget(f"lengths must have shape ({B},), got {tuple(ln.shape)}")
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                          ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq)
+                                          ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq,
+                                          posture_weights=pw)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran
