@@ -365,6 +365,51 @@ int bik_track_weighted_ex64(const bik_problem* problem, int B, int T, double* q,
                             double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
                             int32_t* status, int32_t* passes, void* stream);
 
+/* ---- per-instance joint limits ------------------------------------------------------------------------------------------
+ * The ..._weighted_ex entry points with one more argument, `bounds`, right after `posture_weights`: each instance narrows the
+ * problem's ConfigurationLimit bounds and VelocityLimit caps with its own, as mink's ConfigurationLimit.lower / upper and
+ * VelocityLimit.limit would be changed between two solve_ik calls.  A cap of 0 (or lower == upper == q) locks a dof of one
+ * instance exactly, e.g. the base of a mobile robot on the instances where it must stay put.
+ *   bounds  host memory; its members are device buffers [B][nv] (tangent dofs; bik_track_bounded: one row per instance, used on
+ *           every frame), float or double like the other inputs (bik_inputs.f64), each NULL for no narrowing.  A NULL `bounds`,
+ *           or one whose three members are NULL, runs exactly what the ..._weighted_ex entry point runs, bit for bit.
+ *           `lower` / `upper` on a problem without a ConfigurationLimit, `vmax` on one without a VelocityLimit: BIK_ERR_INVALID.
+ *   `weights` and `posture_weights` as in the ..._weighted_ex entry points, each NULL for none.
+ *   Narrowing only.  For instance b and dof d, every ConfigurationLimit that lists d (gives it a finite bound) gets the bounds
+ *   max(lower_c, lower[b][d]) and min(upper_c, upper[b][d]) and keeps its gain; the VelocityLimit's cap of a dof it lists (a
+ *   finite cap) becomes min(vmax_d, vmax[b][d]).  The values of the other dofs are not read.  So the set of bounded dofs is
+ *   the problem's, and so are the leading unbounded dofs the solver eliminates once: to widen a bound per instance, build the
+ *   problem with the widest bounds and narrow them.  Instance b solves the QP of a problem built with its narrowed bounds; the
+ *   problem stores bounds in fp32, so where the values are exactly representable in fp32 the results are that problem's bit
+ *   for bit (dq, q, iterations, status), otherwise they are used in the caller's precision.  -inf / +inf narrow nothing.  A NaN
+ *   narrows nothing and sets BIK_STATUS_NONFINITE on the instance (bik_track: on the frame in progress).  Narrowing to
+ *   lower > upper, or a negative cap, sets BIK_STATUS_QP_INFEASIBLE, as that problem would.
+ *   BIK_STATUS_OUT_OF_LIMITS and bik_check_limits still test the model's joint range (Configuration.check_limits), and
+ *   bik_limits_box / bik_step_host have no bounded form. */
+typedef struct bik_bounds {
+  const void* lower;   /* [B][nv] or NULL: narrows the ConfigurationLimit bounds of the dofs they list */
+  const void* upper;   /* [B][nv] or NULL */
+  const void* vmax;    /* [B][nv] or NULL: narrows the VelocityLimit caps of the dofs it lists */
+} bik_bounds;          /* element type follows bik_inputs.f64 */
+int bik_step_bounded(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                     const bik_bounds* bounds, float dt, double damping, int nsteps, int integrate, float* dq, int32_t* status, void* stream);
+int bik_converge_bounded(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                         const bik_bounds* bounds, float dt, double damping, int max_iters, float pos_threshold, float ori_threshold,
+                         int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_bounded(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                      const bik_bounds* bounds, const int32_t* lengths, float dt, double damping, int max_iters, float pos_threshold,
+                      float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+int bik_step_bounded64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                       const bik_bounds* bounds, double dt, double damping, int nsteps, int integrate, double* dq, int32_t* status,
+                       void* stream);
+int bik_converge_bounded64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                           const bik_bounds* bounds, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
+                           int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_bounded64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                        const void* posture_weights, const bik_bounds* bounds, const int32_t* lengths, double dt, double damping,
+                        int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
+                        int32_t* status, int32_t* passes, void* stream);
+
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */
 int bik_measure_fma_peak(int device, int use_double, int repeats, double* tflops);

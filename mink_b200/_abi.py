@@ -54,6 +54,10 @@ class BikInputs(C.Structure):
                 ("com_targets", C.c_void_p), ("posture_batched", C.c_int32), ("f64", C.c_int32)]
 
 
+class BikBounds(C.Structure):   # per-instance bounds of the ..._bounded entry points: [B][nv] device buffers or NULL
+    _fields_ = [("lower", C.c_void_p), ("upper", C.c_void_p), ("vmax", C.c_void_p)]
+
+
 class BikDims(C.Structure):
     _fields_ = [("nq", C.c_int32), ("nv", C.c_int32), ("nnode", C.c_int32), ("nframe", C.c_int32),
                 ("nposture", C.c_int32), ("ncom", C.c_int32), ("nrows", C.c_int32), ("npairs", C.c_int32)]

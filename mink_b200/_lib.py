@@ -5,7 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-from ._abi import BikDims, BikFrame, BikInputs, BikLimitDesc, BikTaskDesc
+from ._abi import BikBounds, BikDims, BikFrame, BikInputs, BikLimitDesc, BikTaskDesc
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libbik.so")
 _lib = None
@@ -18,7 +18,8 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_integrate64", "bik_check_limits64", "bik_step64", "bik_converge64", "bik_track64", "bik_measure_fma_peak",
            "bik_step_weighted", "bik_converge_weighted", "bik_track_weighted", "bik_step_weighted64", "bik_converge_weighted64",
            "bik_track_weighted64", "bik_step_weighted_ex", "bik_converge_weighted_ex", "bik_track_weighted_ex",
-           "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64"]
+           "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64", "bik_step_bounded",
+           "bik_converge_bounded", "bik_track_bounded", "bik_step_bounded64", "bik_converge_bounded64", "bik_track_bounded64"]
 
 
 class BikError(RuntimeError):
@@ -87,6 +88,9 @@ def load():
         getattr(lib, name.replace("64", "") + "_weighted" + ("64" if name.endswith("64") else "")).argtypes = args[:at] + [vp] + args[at:]
         # per-instance posture weights: one more pointer after the task weights
         getattr(lib, name.replace("64", "") + "_weighted_ex" + ("64" if name.endswith("64") else "")).argtypes = args[:at] + [vp, vp] + args[at:]
+        # per-instance bounds: a bik_bounds after the posture weights
+        getattr(lib, name.replace("64", "") + "_bounded" + ("64" if name.endswith("64") else "")).argtypes = (args[:at] + [vp, vp, C.POINTER(BikBounds)]
+                                                                                                     + args[at:])
     _lib = lib
     return lib
 

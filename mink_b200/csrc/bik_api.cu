@@ -313,10 +313,15 @@ extern "C" int bik_frame_jacobian64(const bik_model* model, int B, const double*
 }
 
 // track: a bik_track entry point, the only ones that take a posture target sequence
-static int check_inputs(const bik_problem* p, const bik_inputs* in, bool need_q, int f64, bool track = false, const void* posture_weights = nullptr) {
+// bounds: the ..._bounded entry points' bounds (as from bounds_of), or null
+static int check_inputs(const bik_problem* p, const bik_inputs* in, bool need_q, int f64, bool track = false, const void* posture_weights = nullptr,
+                        const bik_bounds* bounds = nullptr) {
   if (!p || !in) return bik_fail(BIK_ERR_INVALID, "null argument");
   const PHeader& h = p->h;
   if (posture_weights && h.P == 0) return bik_fail(BIK_ERR_INVALID, "posture_weights given for a problem without a PostureTask or DampingTask");
+  if (bounds && (bounds->lower || bounds->upper) && h.ncfg == 0)
+    return bik_fail(BIK_ERR_INVALID, "bounds.lower / bounds.upper given for a problem without a ConfigurationLimit");
+  if (bounds && bounds->vmax && !h.has_vel) return bik_fail(BIK_ERR_INVALID, "bounds.vmax given for a problem without a VelocityLimit");
   if (!track && posture_seq(in))
     return bik_fail(BIK_ERR_INVALID, "posture_batched = " + std::to_string(in->posture_batched) +
                                          " (a posture target sequence) is accepted by bik_track, bik_track64 and bik_track_weighted[64] only");
@@ -471,8 +476,10 @@ int HostStaging::reserve(const PHeader& h, size_t B, size_t pt_elems) {
 
 // One or more solve_ik steps on device buffers: per step K1 (check_limits + FK + packed task rows + collision rows) and
 // K2 (QP + integrate).  Caller holds p->mu and has reserved the hand-off for `k1d ? 8 : 4`-byte elements.
-static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, const void* weights, const void* posture_weights, double dt,
-                     double damping, int nsteps, int integrate, void* dq, int32_t* status, int io64, bool k1d, cudaStream_t st) {
+// bounds: per-instance bounds (the bounded K2), or null.
+static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                     const bik_bounds* bounds, double dt, double damping, int nsteps, int integrate, void* dq, int32_t* status, int io64, bool k1d,
+                     cudaStream_t st) {
   // hand-off rows [ws_off, ws_off + B): chunks of one batch may be in flight on different streams (bik_step_host)
   const HandoffSizes n = handoff_sizes(p->h);
   const size_t es = k1d ? 8 : 4;
@@ -497,7 +504,13 @@ static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_in
     a2.B = B; a2.q = q; a2.io64 = io64; a2.pk = pk; a2.pk64 = k1d; a2.ptgt = in->posture_targets; a2.pbatched = in->posture_batched;
     a2.Gc = Gc; a2.hc = hc; a2.gc64 = k1d; a2.dt = dt; a2.damping = damping; a2.dq = dq; a2.integrate = integrate; a2.status = status;
     a2.warm = warm ? warmb : nullptr;
-    if (posture_weights) {
+    if (bounds) {
+      K2BdArgs ba;
+      memset(&ba, 0, sizeof ba);
+      static_cast<K2Args&>(ba) = a2;
+      ba.pw = posture_weights; ba.lower = bounds->lower; ba.upper = bounds->upper; ba.vmax = bounds->vmax;
+      rc = dispatch_k2(p, ba, st);
+    } else if (posture_weights) {
       K2PwArgs pa;
       memset(&pa, 0, sizeof pa);
       static_cast<K2Args&>(pa) = a2;
@@ -511,10 +524,16 @@ static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_in
   return BIK_OK;
 }
 
-static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights, double dt,
-                       double damping, int nsteps, int integrate, void* dq, int32_t* status, int f64, void* stream) {
+// The bounds of a ..._bounded call, or null when it narrows nothing (no struct, or three null members): such a call runs what
+// the ..._weighted_ex call runs.
+static const bik_bounds* bounds_of(const bik_bounds* bounds) { return bounds && has_bounds(*bounds) ? bounds : nullptr; }
+
+static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                       const bik_bounds* bounds, double dt, double damping, int nsteps, int integrate, void* dq, int32_t* status, int f64,
+                       void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, f64, false, posture_weights);
+  bounds = bounds_of(bounds);
+  int rc = check_inputs(cp, in, false, f64, false, posture_weights, bounds);
   if (rc) return rc;
   if (!q || !dq || B < 0 || nsteps < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   bik_problem* p = const_cast<bik_problem*>(cp);
@@ -527,31 +546,41 @@ static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* 
   rc = ws_acquire(p, st);
   if (rc) return rc;
   // (status needs no clearing: K1's fused check_limits assigns it on the first step, everything later ORs into it)
-  return ws_release(p, st, step_core(p, B, 0, q, in, weights, posture_weights, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
+  return ws_release(p, st, step_core(p, B, 0, q, in, weights, posture_weights, bounds, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
 }
 extern "C" int bik_step(const bik_problem* p, int B, float* q, const bik_inputs* in, float dt, double damping, int nsteps, int integrate, float* dq,
                         int32_t* status, void* stream) {
-  return step_common(p, B, q, in, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
+  return step_common(p, B, q, in, nullptr, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
 }
 extern "C" int bik_step64(const bik_problem* p, int B, double* q, const bik_inputs* in, double dt, double damping, int nsteps, int integrate, double* dq,
                           int32_t* status, void* stream) {
-  return step_common(p, B, q, in, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
+  return step_common(p, B, q, in, nullptr, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
 }
 extern "C" int bik_step_weighted(const bik_problem* p, int B, float* q, const bik_inputs* in, const void* weights, float dt, double damping, int nsteps,
                                  int integrate, float* dq, int32_t* status, void* stream) {
-  return step_common(p, B, q, in, weights, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
+  return step_common(p, B, q, in, weights, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
 }
 extern "C" int bik_step_weighted64(const bik_problem* p, int B, double* q, const bik_inputs* in, const void* weights, double dt, double damping,
                                    int nsteps, int integrate, double* dq, int32_t* status, void* stream) {
-  return step_common(p, B, q, in, weights, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
+  return step_common(p, B, q, in, weights, nullptr, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
 }
 extern "C" int bik_step_weighted_ex(const bik_problem* p, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                                     float dt, double damping, int nsteps, int integrate, float* dq, int32_t* status, void* stream) {
-  return step_common(p, B, q, in, weights, posture_weights, dt, damping, nsteps, integrate, dq, status, 0, stream);
+  return step_common(p, B, q, in, weights, posture_weights, nullptr, dt, damping, nsteps, integrate, dq, status, 0, stream);
 }
 extern "C" int bik_step_weighted_ex64(const bik_problem* p, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                                       double dt, double damping, int nsteps, int integrate, double* dq, int32_t* status, void* stream) {
-  return step_common(p, B, q, in, weights, posture_weights, dt, damping, nsteps, integrate, dq, status, 1, stream);
+  return step_common(p, B, q, in, weights, posture_weights, nullptr, dt, damping, nsteps, integrate, dq, status, 1, stream);
+}
+extern "C" int bik_step_bounded(const bik_problem* p, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                const bik_bounds* bounds, float dt, double damping, int nsteps, int integrate, float* dq, int32_t* status,
+                                void* stream) {
+  return step_common(p, B, q, in, weights, posture_weights, bounds, dt, damping, nsteps, integrate, dq, status, 0, stream);
+}
+extern "C" int bik_step_bounded64(const bik_problem* p, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                  const bik_bounds* bounds, double dt, double damping, int nsteps, int integrate, double* dq, int32_t* status,
+                                  void* stream) {
+  return step_common(p, B, q, in, weights, posture_weights, bounds, dt, damping, nsteps, integrate, dq, status, 1, stream);
 }
 
 extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* buf, size_t cap) {
@@ -591,7 +620,8 @@ static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cud
   int rc = bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st);
   if (rc) return rc;
   conv_cond_kernel<<<1, 1, 0, st>>>(c.track, c.max_iters, s.count, handle, use_handle);
-  rc = c.posture_weights ? dispatch_k2(p, conv_k2_pw_args(c, s, status), st) : dispatch_k2(p, conv_k2_args(c, s, status), st);
+  if (has_bounds(c.bounds)) rc = dispatch_k2(p, conv_k2_bd_args(c, s, status), st);
+  else rc = c.posture_weights ? dispatch_k2(p, conv_k2_pw_args(c, s, status), st) : dispatch_k2(p, conv_k2_args(c, s, status), st);
   if (rc) return rc;
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
@@ -690,11 +720,12 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   return ws_release(p, st, BIK_OK);
 }
 
-static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights, double dt,
-                           double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status,
-                           int io64, void* stream) {
+static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                           const bik_bounds* bounds, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
+                           int check_every, int32_t* iters, int32_t* status, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, io64, false, posture_weights);
+  bounds = bounds_of(bounds);
+  int rc = check_inputs(cp, in, false, io64, false, posture_weights, bounds);
   if (rc) return rc;
   if (!q || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (check_every < 1) check_every = 1;
@@ -704,36 +735,49 @@ static int converge_common(const bik_problem* cp, int B, void* q, const bik_inpu
   c.B = B; c.T = 1; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
   c.iters = iters; c.status = status; c.track = false; c.k1d = k1_double(p, damping, io64 != 0, posture_weights != nullptr); c.io64 = io64 != 0;
   c.weights = weights; c.posture_weights = posture_weights;
+  if (bounds) c.bounds = *bounds;
   return converge_run(p, c, check_every, nullptr, static_cast<cudaStream_t>(stream));
 }
 extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
                             float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
+  return converge_common(cp, B, q, in, nullptr, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
 }
 extern "C" int bik_converge64(const bik_problem* cp, int B, double* q, const bik_inputs* in, double dt, double damping, int max_iters,
                               double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
+  return converge_common(cp, B, q, in, nullptr, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
 }
 extern "C" int bik_converge_weighted(const bik_problem* cp, int B, float* q, const bik_inputs* in, const void* weights, float dt, double damping,
                                      int max_iters, float pos_threshold, float ori_threshold, int check_every, int32_t* iters, int32_t* status,
                                      void* stream) {
-  return converge_common(cp, B, q, in, weights, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
+  return converge_common(cp, B, q, in, weights, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0, stream);
 }
 extern "C" int bik_converge_weighted64(const bik_problem* cp, int B, double* q, const bik_inputs* in, const void* weights, double dt, double damping,
                                        int max_iters, double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status,
                                        void* stream) {
-  return converge_common(cp, B, q, in, weights, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
+  return converge_common(cp, B, q, in, weights, nullptr, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1, stream);
 }
 extern "C" int bik_converge_weighted_ex(const bik_problem* cp, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                                         float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every,
                                         int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, weights, posture_weights, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0,
+  return converge_common(cp, B, q, in, weights, posture_weights, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0,
                          stream);
 }
 extern "C" int bik_converge_weighted_ex64(const bik_problem* cp, int B, double* q, const bik_inputs* in, const void* weights,
                                           const void* posture_weights, double dt, double damping, int max_iters, double pos_threshold,
                                           double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
-  return converge_common(cp, B, q, in, weights, posture_weights, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1,
+  return converge_common(cp, B, q, in, weights, posture_weights, nullptr, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1,
+                         stream);
+}
+extern "C" int bik_converge_bounded(const bik_problem* cp, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                    const bik_bounds* bounds, float dt, double damping, int max_iters, float pos_threshold, float ori_threshold,
+                                    int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, weights, posture_weights, bounds, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0,
+                         stream);
+}
+extern "C" int bik_converge_bounded64(const bik_problem* cp, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                      const bik_bounds* bounds, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
+                                      int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, weights, posture_weights, bounds, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1,
                          stream);
 }
 
@@ -741,10 +785,11 @@ extern "C" int bik_converge_weighted_ex64(const bik_problem* cp, int B, double* 
 // One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
 // moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
 static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
-                        const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
-                        void* q_traj, int32_t* iters, int32_t* status, int32_t* passes, int io64, void* stream) {
+                        const bik_bounds* bounds, const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
+                        double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status, int32_t* passes, int io64, void* stream) {
   if (B == 0 && cp) return BIK_OK;
-  int rc = check_inputs(cp, in, false, io64, true, posture_weights);
+  bounds = bounds_of(bounds);
+  int rc = check_inputs(cp, in, false, io64, true, posture_weights, bounds);
   if (rc) return rc;
   if (!q || !q_traj || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (T < 1) return bik_fail(BIK_ERR_INVALID, "T must be at least 1");
@@ -764,44 +809,58 @@ static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_
   c.B = B; c.T = T; c.max_iters = max_iters; c.dt = dt; c.pos = pos_threshold; c.ori = ori_threshold; c.damping = damping; c.q = q; c.in = in;
   c.lengths = lengths; c.q_traj = q_traj; c.iters = iters; c.status = status; c.track = true;
   c.k1d = k1_double(p, damping, io64 != 0, posture_weights != nullptr); c.io64 = io64 != 0; c.weights = weights; c.posture_weights = posture_weights;
+  if (bounds) c.bounds = *bounds;
   return converge_run(p, c, check_every, passes, st);
 }
 extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
                          int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
                          int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 0,
+  return track_common(cp, B, T, q, in, nullptr, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 0,
                       stream);
 }
 extern "C" int bik_track_weighted(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights, const int32_t* lengths,
                                   float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj,
                                   int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, weights, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
+  return track_common(cp, B, T, q, in, weights, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
                       0, stream);
 }
 extern "C" int bik_track_weighted64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights, const int32_t* lengths,
                                     double dt, double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every,
                                     double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, weights, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
+  return track_common(cp, B, T, q, in, weights, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes,
                       1, stream);
 }
 extern "C" int bik_track_weighted_ex(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights,
                                      const void* posture_weights, const int32_t* lengths, float dt, double damping, int max_iters, float pos_threshold,
                                      float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status, int32_t* passes,
                                      void* stream) {
-  return track_common(cp, B, T, q, in, weights, posture_weights, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+  return track_common(cp, B, T, q, in, weights, posture_weights, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
                       iters, status, passes, 0, stream);
 }
 extern "C" int bik_track_weighted_ex64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights,
                                        const void* posture_weights, const int32_t* lengths, double dt, double damping, int max_iters,
                                        double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters, int32_t* status,
                                        int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, weights, posture_weights, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+  return track_common(cp, B, T, q, in, weights, posture_weights, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 1, stream);
+}
+extern "C" int bik_track_bounded(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                 const bik_bounds* bounds, const int32_t* lengths, float dt, double damping, int max_iters, float pos_threshold,
+                                 float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 0, stream);
+}
+extern "C" int bik_track_bounded64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                                   const void* posture_weights, const bik_bounds* bounds, const int32_t* lengths, double dt, double damping,
+                                   int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
+                                   int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
                       iters, status, passes, 1, stream);
 }
 extern "C" int bik_track64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
                            int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
                            int32_t* status, int32_t* passes, void* stream) {
-  return track_common(cp, B, T, q, in, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 1,
+  return track_common(cp, B, T, q, in, nullptr, nullptr, nullptr, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj, iters, status, passes, 1,
                       stream);
 }
 
@@ -891,7 +950,7 @@ extern "C" int bik_step_host(const bik_problem* cp, int B, float* q_host, const 
     bik_inputs din = *in;
     din.q = hq + o * nq; din.frame_targets = hft + o * h.F * 7; din.com_targets = hct + o * h.C * 3;
     din.posture_targets = in->posture_batched ? hpt + o * (size_t)h.P * nq : hpt;
-    rc = step_core(p, (int)n, o, hq + o * nq, &din, nullptr, nullptr, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
+    rc = step_core(p, (int)n, o, hq + o * nq, &din, nullptr, nullptr, nullptr, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
     if (rc) return rc;
     CUDA_OK(cudaEventRecord(hb.hev[2 * ci + 1], s_cmp));
     mark(s_cmp);

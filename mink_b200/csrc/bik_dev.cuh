@@ -182,9 +182,11 @@ int bik_launch_k1(const bik_problem* p, const bik::K1Args& a, bool use_double, c
 int bik_launch_fk(const bik_model* m, const bik::FkArgs& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2Args& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2PwArgs& a, cudaStream_t st);   // posture-weighted instantiations
+int bik_launch_k2_general(const bik_problem* p, const bik::K2BdArgs& a, cudaStream_t st);   // bounded instantiations
 void bik_k2_general_shape(const bik_problem* p, int* lanes, int* slots);   // the (W, SLOTS) bik_launch_k2_general picks
 int bik_launch_k2_group(const bik_problem* p, const bik::K2Args& a, unsigned int* sched, cudaStream_t st);
 int bik_launch_k2_group(const bik_problem* p, const bik::K2PwArgs& a, unsigned int* sched, cudaStream_t st);   // posture-weighted
+int bik_launch_k2_group(const bik_problem* p, const bik::K2BdArgs& a, unsigned int* sched, cudaStream_t st);   // bounded
 bool bik_k2_group_applies(const bik_problem* p);                  // box-only, at most 64 coupled dofs, fits in shared memory
 long long bik_k2_group_wave(const bik_problem* p);                // instances one resident wave of the small-group K2 covers
 const char* bik_k2_describe(const bik_problem* p, char* buf, size_t cap);

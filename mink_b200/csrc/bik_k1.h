@@ -1127,20 +1127,61 @@ BIK_HD int check_limits_instance(const PView& P, const T* q, float tol) {  // co
   }
   return bad;
 }
-// lo <= dq <= hi from ConfigurationLimit(s) and VelocityLimit (configuration_limit.py:98-124, velocity_limit.py:99-101);
-// qi = q of the dof (unused for free / ball dofs)
+// ---- per-instance bounds (the ..._bounded entry points) ---------------------------------------------------------------
+// One instance's rows of the caller's [B][nv] lower / upper / vmax buffers, each null when not given; element type by is64.
+// A null row, or a BoundsRow of null rows, narrows nothing.
+struct BoundsRow { const void *lo, *up, *vm; int is64; };
+// The problem's bound `tab` of dof d narrowed by the instance's value in `row`: the larger of the two for a lower bound, the
+// smaller for an upper bound or a cap.  `tab` itself for a null row, or for a NaN value, which sets BIK_STATUS_NONFINITE (4)
+// in *st.  The callers narrow only the bounds the problem gives a dof, so the set of bounded dofs never changes.
+template <typename T, bool UPPER>
+BIK_HD T bd_narrow(T tab, const void* row, int d, int is64, int* st) {
+  if (!row) return tab;
+  const T v = ldin<T>(row, d, is64);
+  if (!(v == v)) { *st |= 4; return tab; }
+  return UPPER ? bik_min(tab, v) : bik_max(tab, v);
+}
+// ConfigurationLimit c lists the dof (gives it a finite bound): its bounds [lc, uc] are narrowed by the instance's
 template <typename T>
-BIK_HD void box_dof(const PView& P, int d, T qi, T dt, T* lo, T* hi) {
+BIK_HD void bd_narrow_cfg(const BoundsRow& bd, int d, T* lc, T* uc, int* st) {
+  if (*lc > -T(BIK_INF_F) || *uc < T(BIK_INF_F)) {
+    *lc = bd_narrow<T, false>(*lc, bd.lo, d, bd.is64, st);
+    *uc = bd_narrow<T, true>(*uc, bd.up, d, bd.is64, st);
+  }
+}
+// the VelocityLimit lists the dof (gives it a finite cap): the cap is narrowed by the instance's
+template <typename T>
+BIK_HD T bd_narrow_vmax(const BoundsRow& bd, int d, T vmax, int* st) {
+  return vmax < T(BIK_INF_F) ? bd_narrow<T, true>(vmax, bd.vm, d, bd.is64, st) : vmax;
+}
+
+// lo <= dq <= hi from ConfigurationLimit(s) and VelocityLimit (configuration_limit.py:98-124, velocity_limit.py:99-101);
+// qi = q of the dof (unused for free / ball dofs).  BD (compile time): the instance's bounds `bd` narrow the problem's before
+// they enter the same products (NaN bounds set BIK_STATUS_NONFINITE in *st), so bounds equal to the problem's give its bits.
+template <typename T, bool BD = false>
+BIK_HD void box_dof(const PView& P, int d, T qi, T dt, T* lo, T* hi, const BoundsRow* bd = nullptr, int* st = nullptr) {
   const PHeader& h = P.h();
   T l = -T(BIK_INF_F), u = T(BIK_INF_F);
   if (P.i(h.off_dofqadr)[d] >= 0) {
     for (int c = 0; c < h.ncfg; ++c) {
       const float* p = P.f(h.off_cfg) + c * (2 + 2 * h.nv);
-      T up = T(p[0]) * (T(p[2 + h.nv + d]) - qi), dn = T(p[0]) * (qi - T(p[2 + d]));
+      T up, dn;
+      if constexpr (BD) {
+        T lc = T(p[2 + d]), uc = T(p[2 + h.nv + d]);
+        bd_narrow_cfg<T>(*bd, d, &lc, &uc, st);
+        up = T(p[0]) * (uc - qi); dn = T(p[0]) * (qi - lc);
+      } else {
+        up = T(p[0]) * (T(p[2 + h.nv + d]) - qi); dn = T(p[0]) * (qi - T(p[2 + d]));
+      }
       u = bik_min(u, up); l = bik_max(l, -dn);
     }
   }
-  if (h.has_vel) { T vm = dt * T(P.f(h.off_vmax)[d]); u = bik_min(u, vm); l = bik_max(l, -vm); }
+  if (h.has_vel) {
+    T vm;
+    if constexpr (BD) vm = dt * bd_narrow_vmax<T>(*bd, d, T(P.f(h.off_vmax)[d]), st);
+    else vm = dt * T(P.f(h.off_vmax)[d]);
+    u = bik_min(u, vm); l = bik_max(l, -vm);
+  }
   *lo = l; *hi = u;
 }
 

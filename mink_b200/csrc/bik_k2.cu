@@ -5,7 +5,7 @@ using namespace bik;
 
 // W lanes per problem (32 / W problems per warp): 8 or 16 when the augmented factor (coupled dofs + right-hand side) has at most
 // that many rows -- a 6-dof arm with collision rows leaves 26 of 32 lanes idle with a warp per problem.
-template <int W, int SLOTS, bool PW>
+template <int W, int SLOTS, bool PW, bool BD = false>
 __device__ __forceinline__ void k2_problems(const uint32_t* __restrict__ gimage, int words, int use_tma, const K2Args& a) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ __align__(8) uint64_t bar;
@@ -17,7 +17,7 @@ __device__ __forceinline__ void k2_problems(const uint32_t* __restrict__ gimage,
   const int grp = lane32 / W, lane = lane32 % W;
   char* wsm = reinterpret_cast<char*>(smem + words) + (size_t)(warp * PPW + grp) * k2_warp_bytes(P.h(), sizeof(double));
   for (long long b = (long long)(blockIdx.x * nwarps + warp) * PPW + grp; b < a.B; b += (long long)gridDim.x * nwarps * PPW)
-    k2_warp<double, W, SLOTS, PW>(P, a, (int)b, wsm, lane);
+    k2_warp<double, W, SLOTS, PW, BD>(P, a, (int)b, wsm, lane);
 }
 template <int W, int SLOTS>
 __global__ void __launch_bounds__(256) k2_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2Args a) {
@@ -28,11 +28,16 @@ template <int W, int SLOTS>
 __global__ void __launch_bounds__(256) k2_pw_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2PwArgs a) {
   k2_problems<W, SLOTS, true>(gimage, words, use_tma, a);
 }
+// The same with per-instance bounds and posture weights, which may be null (K2BdArgs): the ..._bounded entry points with bounds.
+template <int W, int SLOTS>
+__global__ void __launch_bounds__(256) k2_bd_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K2BdArgs a) {
+  k2_problems<W, SLOTS, true, true>(gimage, words, use_tma, a);
+}
 
-// A: K2Args (k2_kernel) or K2PwArgs (k2_pw_kernel)
+// A: K2Args (k2_kernel), K2PwArgs (k2_pw_kernel) or K2BdArgs (k2_bd_kernel)
 template <int W, int SLOTS, typename A>
 static int launch_k2(const bik_problem* p, const A& a, cudaStream_t st) {
-  constexpr bool PW = std::is_same<A, K2PwArgs>::value;
+  constexpr bool PW = std::is_same<A, K2PwArgs>::value, BD = std::is_same<A, K2BdArgs>::value;
   const PHeader& h = p->h;
   constexpr int PPW = 32 / W;
   int NW = p->k2_warps;
@@ -41,10 +46,11 @@ static int launch_k2(const bik_problem* p, const A& a, cudaStream_t st) {
   size_t smem = need(NW);
   int grid = 1;
   const long long per_cta = (long long)NW * PPW;
-  const void* kern = PW ? (const void*)k2_pw_kernel<W, SLOTS> : (const void*)k2_kernel<W, SLOTS>;
+  const void* kern = BD ? (const void*)k2_bd_kernel<W, SLOTS> : PW ? (const void*)k2_pw_kernel<W, SLOTS> : (const void*)k2_kernel<W, SLOTS>;
   int rc = bik_launch_geometry(kern, p->model, smem, 32 * NW, ((long long)a.B + per_cta - 1) / per_cta, &grid);
   if (rc) return rc;
-  if constexpr (PW) k2_pw_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
+  if constexpr (BD) k2_bd_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
+  else if constexpr (PW) k2_pw_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
   else k2_kernel<W, SLOTS><<<grid, 32 * NW, smem, st>>>(p->d_image, h.words32, p->model->use_tma, a);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
@@ -66,3 +72,4 @@ static int launch_k2_shape(const bik_problem* p, const A& a, cudaStream_t st) {
 }
 int bik_launch_k2_general(const bik_problem* p, const K2Args& a, cudaStream_t st) { return launch_k2_shape(p, a, st); }
 int bik_launch_k2_general(const bik_problem* p, const K2PwArgs& a, cudaStream_t st) { return launch_k2_shape(p, a, st); }
+int bik_launch_k2_general(const bik_problem* p, const K2BdArgs& a, cudaStream_t st) { return launch_k2_shape(p, a, st); }

@@ -88,6 +88,14 @@ struct K2PwArgs : K2Args {
   const int32_t* pw_cursor;   // [B] or null (step / converge)
   int pw_T;
 };
+// The arguments of the bounded instantiations (BD; the ..._bounded entry points): K2PwArgs, whose posture weights may be null
+// here, and the per-instance bounds.  Each is [B][nv] or null, element type follows io64; in track mode too, row b holds on
+// every frame.  They narrow the problem's ConfigurationLimit bounds and VelocityLimit caps (box_dof).
+struct K2BdArgs : K2PwArgs {
+  const void* lower;
+  const void* upper;
+  const void* vmax;
+};
 
 enum { K2_MAX_GEN = 24 };  // general (collision) rows that may be active at once; more than that sets BIK_STATUS_QP_MAXITER
 
@@ -222,6 +230,14 @@ BIK_HD T k2_pw(const void* pw, long long i, int is64, int* st) {
   if (!(w >= T(0) && w <= T(1))) *st |= 32;
   return w >= T(0) ? (w <= T(1) ? w : T(1)) : T(0);
 }
+// ---- per-instance bounds (K2BdArgs) --------------------------------------------------------------------------------------
+// instance b's rows of the bound buffers.  `a` is the K2BdArgs a BD instantiation was launched with.
+BIK_HD BoundsRow k2_bd_row(const K2Args& a, int nv, long long b, int is64) {
+  const K2BdArgs& ba = static_cast<const K2BdArgs&>(a);
+  const long long off = b * nv * (is64 ? 8 : 4);
+  auto row = [&](const void* p) -> const void* { return p ? reinterpret_cast<const char*>(p) + off : nullptr; };
+  return BoundsRow{row(ba.lower), row(ba.upper), row(ba.vmax), is64};
+}
 
 // One task of the stacked objective: rows, non-zero columns and where its block sits in the packed record.
 struct K2Task { int row0, nr, nc, coff, pk_off; const float* cost; float gain, lm; };
@@ -240,7 +256,8 @@ BIK_HD K2Task k2_task(const PView& P, int t) {
 // ---- assembly ------------------------------------------------------------------------------
 // PW (compile time): per-instance posture weights (K2PwArgs, which `a` then is): the cost of posture task p on dof d is
 // cost_eff[d] * w.
-template <typename T, int W, bool PW = false>
+// BD (compile time, with PW): per-instance bounds (K2BdArgs, which `a` then is) narrow the box; the posture weights may be null.
+template <typename T, int W, bool PW = false, bool BD = false>
 BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int lane) {
   const PHeader& h = P.h();
   const int n = h.nv, nu = h.nu, K = h.K, nq = h.nq;
@@ -307,14 +324,14 @@ BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int l
     return posture_err_dof<T>(P, d, [&](int i) { return ldin<T>(a.ptgt, t0 + i, a.io64); }, qv);
   };
   const void* pw = nullptr;
-  if constexpr (PW) pw = k2_pw_row(a, h, b, a.io64);
+  if constexpr (PW) if (!BD || static_cast<const K2PwArgs&>(a).pw) pw = k2_pw_row(a, h, b, a.io64);
   for (int p = 0; p < h.P; ++p) {
     const float* pr = P.f(h.off_posture) + p * (2 + n);
     if (pr[1] != 0.f) {
       T s = T(0);
       for (int d = lane; d < n; d += W) {
         T wgt = T(pr[2 + d]);
-        if constexpr (PW) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
+        if constexpr (PW) if (!BD || pw) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
         T v = wgt * T(pr[0]) * eperr(p, d);
         s += v * v;
       }
@@ -324,18 +341,20 @@ BIK_HD int k2_assemble(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int l
   }
   // diagonal, posture part of the linear term and box.  A DECOUPLED dof (zero column in every task Jacobian) only sees
   // the diagonal: its optimum is the clamp of -c/h, written straight to xfull.
+  BoundsRow bd{};
+  if constexpr (BD) bd = k2_bd_row(a, n, b, a.io64);
   for (int d = lane; d < n; d += W) {
     const int u = umap[d];
     T cd = T(0), hd = mu;
     for (int p = 0; p < h.P; ++p) {
       const float* pr = P.f(h.off_posture) + p * (2 + n);
       T wgt = T(pr[2 + d]);
-      if constexpr (PW) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
+      if constexpr (PW) if (!BD || pw) wgt *= k2_pw<T>(pw, p * n + d, a.io64, &status);
       hd += wgt * wgt;                                  // (W J)^T (W J), J = -I
       if (wgt != T(0)) cd -= T(pr[0]) * wgt * wgt * eperr(p, d);  // -(W(-g e))^T W (-I)
     }
     T lo = -T(BIK_INF_F), hi = T(BIK_INF_F);
-    if (!a.skip_box) { const int qa = dofqadr[d]; box_dof<T>(P, d, qa >= 0 ? qv(qa) : T(0), T(a.dt), &lo, &hi); }
+    if (!a.skip_box) { const int qa = dofqadr[d]; box_dof<T, BD>(P, d, qa >= 0 ? qv(qa) : T(0), T(a.dt), &lo, &hi, &bd, &status); }
     if (a.lo_out) { stout<T>(a.lo_out, (long long)b * n + d, a.io64, lo); stout<T>(a.hi_out, (long long)b * n + d, a.io64, hi); }
     if (lo > hi + T(1e-9) * (T(1) + (hi < 0 ? -hi : hi))) status |= 8;   // inconsistent limits (e.g. a configuration far outside its range with a velocity limit): the reference's QP has no solution (solve_ik.py:103)
     if (u >= 0) {
@@ -753,14 +772,14 @@ BIK_HD int k2_solve(const PView& P, const K2Args& a, int b, K2Ws<T>& w, int lane
 }
 
 // One instance per warp: assemble, optionally dump (H, c) / (lo, hi), solve, write dq, optionally integrate q.
-template <typename T, int W, int SLOTS, bool PW = false>
+template <typename T, int W, int SLOTS, bool PW = false, bool BD = false>
 BIK_HD void k2_warp(const PView& P, const K2Args& a, int b, void* wsm, int lane) {
   const PHeader& h = P.h();
   const int n = h.nv, nu = h.nu, nq = h.nq;
   const int32_t* umap = P.i(h.off_umap);
   if (a.skip && a.skip[b]) return;
   K2Ws<T> w = k2_carve<T>(h, wsm);
-  int st = k2_assemble<T, W, PW>(P, a, b, w, lane);
+  int st = k2_assemble<T, W, PW, BD>(P, a, b, w, lane);
   if (a.skip_objective) return;
   if (a.Hout) {
     for (int k = lane; k < n * n; k += W) {

@@ -17,7 +17,7 @@ using namespace bik;
 constexpr int K2T_MAXT = 256;   // threads per CTA at most; two CTAs per SM
 
 // The body of both kernels: tiles from the counter, or round-robin.
-template <typename T, int G, typename M, bool F32IO, bool STEP, bool PW>
+template <typename T, int G, typename M, bool F32IO, bool STEP, bool PW, bool BD = false>
 __device__ __forceinline__ void k2t_tiles(const uint32_t* __restrict__ gimage, int warp_bytes, const K2Args& a, unsigned int* sched) {
   extern __shared__ __align__(16) uint32_t smem[];
   constexpr int NS = 32 / G;
@@ -33,14 +33,14 @@ __device__ __forceinline__ void k2t_tiles(const uint32_t* __restrict__ gimage, i
       if (lane == 0) t = atomicAdd(&sched[0], 1u);
       t = __shfl_sync(0xffffffffu, t, 0);
       if ((long long)t >= ntiles) break;
-      k2t_warp_tile<T, G, NS, M, F32IO, STEP, PW>(P, a, (long long)t * NS, wsm, lane, St, uw);
+      k2t_warp_tile<T, G, NS, M, F32IO, STEP, PW, BD>(P, a, (long long)t * NS, wsm, lane, St, uw);
     }
     __syncthreads();
     if (threadIdx.x == 0 && atomicInc(&sched[1], gridDim.x - 1) == gridDim.x - 1) { __threadfence(); sched[0] = 0u; }
     return;
   }
   for (long long tile = (long long)blockIdx.x * nwarps + warp; tile < ntiles; tile += (long long)gridDim.x * nwarps)
-    k2t_warp_tile<T, G, NS, M, F32IO, STEP, PW>(P, a, tile * NS, wsm, lane, St, uw);
+    k2t_warp_tile<T, G, NS, M, F32IO, STEP, PW, BD>(P, a, tile * NS, wsm, lane, St, uw);
 }
 // Launched as k2t_kernel<double, G, K2T_MAXT, ...> only; T and MAXT stay in the template, and so in the kernel's symbol.
 template <typename T, int G, int MAXT, typename M, bool F32IO, bool STEP>
@@ -52,6 +52,11 @@ template <typename T, int G, int MAXT, typename M, bool F32IO, bool STEP>
 __global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_pw_kernel(const uint32_t* __restrict__ gimage, int warp_bytes, K2PwArgs a, unsigned int* sched) {
   k2t_tiles<T, G, M, F32IO, STEP, true>(gimage, warp_bytes, a, sched);
 }
+// The same with per-instance bounds and posture weights, which may be null (K2BdArgs): the ..._bounded entry points with bounds.
+template <typename T, int G, int MAXT, typename M, bool F32IO, bool STEP>
+__global__ void __launch_bounds__(MAXT, 512 / MAXT) k2t_bd_kernel(const uint32_t* __restrict__ gimage, int warp_bytes, K2BdArgs a, unsigned int* sched) {
+  k2t_tiles<T, G, M, F32IO, STEP, true, true>(gimage, warp_bytes, a, sched);
+}
 
 // warps per CTA: as many as shared memory holds, at most K2T_MAXT / 32
 static int k2t_warps(const bik_problem* p, size_t wb) {
@@ -59,11 +64,11 @@ static int k2t_warps(const bik_problem* p, size_t wb) {
   while (NW > 1 && NW * wb > (size_t)p->model->max_smem) --NW;
   return NW;
 }
-// A: K2Args (k2t_kernel) or K2PwArgs (k2t_pw_kernel)
+// A: K2Args (k2t_kernel), K2PwArgs (k2t_pw_kernel) or K2BdArgs (k2t_bd_kernel)
 template <int G, typename M, bool F32IO, bool STEP, typename A>
 static int launch_k2t_io(const bik_problem* p, const A& a, unsigned int* sched, cudaStream_t st) {
   constexpr int NS = 32 / G;
-  constexpr bool PW = std::is_same<A, K2PwArgs>::value;
+  constexpr bool PW = std::is_same<A, K2PwArgs>::value, BD = std::is_same<A, K2BdArgs>::value;
   PView P{p->image.data()};
   const size_t wb = (size_t)k2t_warp_bytes(P, sizeof(double), NS);
   const int NW = k2t_warps(p, wb);
@@ -71,22 +76,29 @@ static int launch_k2t_io(const bik_problem* p, const A& a, unsigned int* sched, 
   int grid = 1;
   long long tiles = ((long long)a.B + NS - 1) / NS;
   const void* kern;
-  if constexpr (PW) kern = (const void*)k2t_pw_kernel<double, G, K2T_MAXT, M, F32IO, STEP>;
+  if constexpr (BD) kern = (const void*)k2t_bd_kernel<double, G, K2T_MAXT, M, F32IO, STEP>;
+  else if constexpr (PW) kern = (const void*)k2t_pw_kernel<double, G, K2T_MAXT, M, F32IO, STEP>;
   else kern = (const void*)k2t_kernel<double, G, K2T_MAXT, M, F32IO, STEP>;
   int rc = bik_launch_geometry(kern, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
   if (rc) return rc;
-  if constexpr (PW) k2t_pw_kernel<double, G, K2T_MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
+  if constexpr (BD) k2t_bd_kernel<double, G, K2T_MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
+  else if constexpr (PW) k2t_pw_kernel<double, G, K2T_MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
   else k2t_kernel<double, G, K2T_MAXT, M, F32IO, STEP><<<grid, 32 * NW, smem, st>>>(p->d_image, (int)wb, a, sched);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
-template <int G, typename M>
-static int launch_k2t(const bik_problem* p, const K2PwArgs& a, unsigned int* sched, cudaStream_t st) {
-  // posture weights: only the packed forms that bik_step / bik_converge / bik_track launch are instantiated
-  if (!a.pk || a.dense64) return bik_fail(BIK_ERR_UNSUPPORTED, "posture weights need the packed task rows of bik_step / bik_converge / bik_track");
+// posture weights or bounds (A: K2PwArgs or K2BdArgs): only the packed forms that bik_step / bik_converge / bik_track launch are
+// instantiated
+template <int G, typename M, typename A>
+static int launch_k2t_packed(const bik_problem* p, const A& a, unsigned int* sched, cudaStream_t st) {
+  if (!a.pk || a.dense64) return bik_fail(BIK_ERR_UNSUPPORTED, "posture weights and bounds need the packed task rows of bik_step / bik_converge / bik_track");
   if (a.io64 || a.pk64) return launch_k2t_io<G, M, false, false>(p, a, sched, st);
   return launch_k2t_io<G, M, true, true>(p, a, sched, st);
 }
+template <int G, typename M>
+static int launch_k2t(const bik_problem* p, const K2PwArgs& a, unsigned int* sched, cudaStream_t st) { return launch_k2t_packed<G, M>(p, a, sched, st); }
+template <int G, typename M>
+static int launch_k2t(const bik_problem* p, const K2BdArgs& a, unsigned int* sched, cudaStream_t st) { return launch_k2t_packed<G, M>(p, a, sched, st); }
 template <int G, typename M>
 static int launch_k2t(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) {
   if (a.io64 || a.pk64 || a.dense64) return launch_k2t_io<G, M, false, false>(p, a, sched, st);
@@ -118,6 +130,7 @@ static int launch_k2t_group(const bik_problem* p, const A& a, unsigned int* sche
 }
 int bik_launch_k2_group(const bik_problem* p, const K2Args& a, unsigned int* sched, cudaStream_t st) { return launch_k2t_group(p, a, sched, st); }
 int bik_launch_k2_group(const bik_problem* p, const K2PwArgs& a, unsigned int* sched, cudaStream_t st) { return launch_k2t_group(p, a, sched, st); }
+int bik_launch_k2_group(const bik_problem* p, const K2BdArgs& a, unsigned int* sched, cudaStream_t st) { return launch_k2t_group(p, a, sched, st); }
 const char* bik_k2_describe(const bik_problem* p, char* buf, size_t cap) {
   if (bik_k2_group_applies(p)) snprintf(buf, cap, "small-group G=%d%s", group_of(p), p->h.nu > K2T_NMAX ? " (64-bit masks)" : "");
   else {

@@ -443,18 +443,32 @@ BIK_HD void k2t_prefetch_l2(const void* p, int bytes, int l) {
   (void)p; (void)bytes; (void)l;
 #endif
 }
-// box_dof (bik_k1.h) from the dof's record: the same bounds, combined in the same order
-template <typename T>
-BIK_HD void k2t_box_dof(const K2DofRec& r, int ncfg, int has_vel, T qi, T dt, T* lo, T* hi) {
+// box_dof (bik_k1.h) from the dof's record: the same bounds, combined in the same order, narrowed as there (BD: dof d of the
+// instance's bounds `bd`)
+template <typename T, bool BD = false>
+BIK_HD void k2t_box_dof(const K2DofRec& r, int ncfg, int has_vel, T qi, T dt, T* lo, T* hi, const BoundsRow* bd = nullptr, int d = 0,
+                        int* st = nullptr) {
   T l = -T(BIK_INF_F), u = T(BIK_INF_F);
   if (r.qa >= 0) {
     #pragma unroll 1
     for (int c = 0; c < ncfg; ++c) {
-      T up = T(r.cfg[c][0]) * (T(r.cfg[c][2]) - qi), dn = T(r.cfg[c][0]) * (qi - T(r.cfg[c][1]));
+      T up, dn;
+      if constexpr (BD) {
+        T lc = T(r.cfg[c][1]), uc = T(r.cfg[c][2]);
+        bd_narrow_cfg<T>(*bd, d, &lc, &uc, st);
+        up = T(r.cfg[c][0]) * (uc - qi); dn = T(r.cfg[c][0]) * (qi - lc);
+      } else {
+        up = T(r.cfg[c][0]) * (T(r.cfg[c][2]) - qi); dn = T(r.cfg[c][0]) * (qi - T(r.cfg[c][1]));
+      }
       u = bik_min(u, up); l = bik_max(l, -dn);
     }
   }
-  if (has_vel) { T vm = dt * T(r.vmax); u = bik_min(u, vm); l = bik_max(l, -vm); }
+  if (has_vel) {
+    T vm;
+    if constexpr (BD) vm = dt * bd_narrow_vmax<T>(*bd, d, T(r.vmax), st);
+    else vm = dt * T(r.vmax);
+    u = bik_min(u, vm); l = bik_max(l, -vm);
+  }
   *lo = l; *hi = u;
 }
 // q <- q (+) dq of one free or ball joint (quaternion update)
@@ -476,7 +490,9 @@ BIK_NOINLINE void k2t_store_warm(signed char* wm, int nu, M lom, M upm) {
 // PW (compile time): per-instance posture weights (K2PwArgs, which `a` then is; the ..._weighted_ex entry points): the tabled coefficients of
 // posture task p on dof d are scaled by the instance's weight (w^2 and (gain w) w by its square) before they enter the same
 // sums in the same order, so a weight of 1 gives the bits of the unweighted instantiation.
-template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false, bool PW = false>
+// BD (compile time, with PW): per-instance bounds (K2BdArgs, which `a` then is) narrow each dof's box where it is formed
+// (k2t_box_dof); the posture weights may be null.  The decoupled dofs' clamp and the active-set iterations read the same box.
+template <typename T, int G, int NS, typename M = uint32_t, bool F32IO = false, bool STEP = false, bool PW = false, bool BD = false>
 BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* wsm, int lane, int St = 0, int uw = 0) {
   static_assert(!STEP || F32IO, "the step instantiation reads fp32 buffers");
   if (St == 0) { St = k2t_task_tile_words(P); uw = k2t_union_words(P); }   // callers that loop over tiles pass them in
@@ -494,9 +510,17 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
   // PW: this instance's posture weights (null for a slot without a live instance: its results are not stored)
   const void* pw = nullptr;
   if constexpr (PW) {
-    if (live && NP > 0) {
+    if (live && NP > 0 && (!BD || static_cast<const K2PwArgs&>(a).pw)) {
       pw = k2_pw_row(a, h, b, io64);
       k2t_prefetch_l2<G>(pw, NP * nv * (io64 ? 8 : 4), l);
+    }
+  }
+  // BD: this instance's bound rows (null rows for a slot without a live instance), fetched into L2 like the posture weights
+  BoundsRow bd{};
+  if constexpr (BD) {
+    if (live) {
+      bd = k2_bd_row(a, nv, b, io64);
+      for (const void* r : {bd.lo, bd.up, bd.vm}) if (r) k2t_prefetch_l2<G>(r, nv * (io64 ? 8 : 4), l);
     }
   }
   T* const Tb = reinterpret_cast<T*>(wsm);
@@ -567,7 +591,7 @@ BIK_HD void k2t_warp_tile(const PView& P, const K2Args& a, long long b0, void* w
         }
       }
       T bl, bu;
-      k2t_box_dof<T>(dr, h.ncfg, h.has_vel, dr.qa >= 0 ? qrow[dr.qa] : T(0), T(a.dt), &bl, &bu);
+      k2t_box_dof<T, BD>(dr, h.ncfg, h.has_vel, dr.qa >= 0 ? qrow[dr.qa] : T(0), T(a.dt), &bl, &bu, &bd, d, &st);
       if (bl > bu + T(1e-9) * (T(1) + (bu < 0 ? -bu : bu))) st |= 8;   // inconsistent limits: the reference's QP has no solution (solve_ik.py:103)
       if (u >= 0) { Hp[(tri(u) + u) * NS] += hd; c[u * NS] += cd; lo[u * NS] = float(bl); hi[u * NS] = float(bu); }
       else {

@@ -15,11 +15,13 @@ namespace bik {
 // The arguments of one bik_converge / bik_track call.  io64: fp64 buffers (bik_converge64 / bik_track64).  k1d: K1 runs in
 // fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.  weights: the ..._weighted entry
 // points' per-instance task weights (K1Args::weights), or null.  posture_weights: the ..._weighted_ex entry points' per-instance
-// posture weights (K2PwArgs), or null.
+// posture weights (K2PwArgs), or null.  bounds: the ..._bounded entry points' per-instance bounds (K2BdArgs), all three null
+// for none; held by value, so that the converge graph's key holds the three pointers.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
-  void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights;
+  void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights; bik_bounds bounds;
 };
+inline bool has_bounds(const bik_bounds& bd) { return bd.lower || bd.upper || bd.vmax; }
 
 // The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
 // the caller's precision.  warm: [B][max(nu,1)] active-set guess.  done: [B] K2 leaves the instance alone.  cursor / step /
@@ -80,6 +82,14 @@ inline K2PwArgs conv_k2_pw_args(const ConvCall& c, const ConvBufs& s, int32_t* s
   static_cast<K2Args&>(a) = conv_k2_args(c, s, status);
   a.pw = c.posture_weights;
   if (c.track) { a.pw_cursor = s.cursor; a.pw_T = c.T; }
+  return a;
+}
+// The same for the bounded K2 (has_bounds(c.bounds)); the posture weights may be null.  Track mode reads row b on every frame.
+inline K2BdArgs conv_k2_bd_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  K2BdArgs a;
+  memset(&a, 0, sizeof a);
+  static_cast<K2PwArgs&>(a) = conv_k2_pw_args(c, s, status);
+  a.lower = c.bounds.lower; a.upper = c.bounds.upper; a.vmax = c.bounds.vmax;
   return a;
 }
 

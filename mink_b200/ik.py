@@ -14,8 +14,8 @@ import numpy as np
 
 from ._abi import ProblemSpec
 from .configuration import Configuration
-from .exceptions import InvalidTarget
-from .limits import ConfigurationLimit, Limit
+from .exceptions import InvalidTarget, LimitDefinitionError
+from .limits import ConfigurationLimit, Limit, VelocityLimit
 from .tasks import ComTask, DampingTask, FrameTask, PostureTask, Task, problem_for
 
 
@@ -135,6 +135,52 @@ def _posture_weights(tasks: Sequence[Task], posture_weights, q, nv: int, T: Opti
     return torch.stack(blocks, dim=-2).contiguous()
 
 
+def _limit_bounds(limits: Optional[Sequence[Limit]], bounds, q, flat):
+    """The (lower, upper, vmax) [B, nv] buffers of a `bounds={limit: value}` mapping, +-inf where nothing narrows; None for no
+    mapping.  `limits` is the caller's list (None: the implicit default, which no key can name).
+    ConfigurationLimit: (lower, upper), each None, [nq] or [B, nq] by qpos address; only the limit's listed dofs are read.
+    VelocityLimit: vmax [k] or [B, k] in the order of limit.indices."""
+    if not bounds:
+        return None
+    import torch
+
+    B, nq, nv = q.shape[0], flat.nq, flat.nv
+    listed = list(limits or [])
+    full = lambda v: torch.full((B, nv), v, device=q.device, dtype=q.dtype)
+    lo = up = vm = None
+
+    def rows(x, n, what):
+        x = x if isinstance(x, torch.Tensor) else torch.as_tensor(np.array(x, dtype=np.float64))
+        x = x.to(device=q.device, dtype=q.dtype)
+        if tuple(x.shape) not in ((n,), (B, n)):
+            raise LimitDefinitionError(f"Expected {what} of shape [{n}] or [{B}, {n}], got {list(x.shape)}")
+        return x.expand(B, n)
+
+    for limit, value in bounds.items():
+        if not isinstance(limit, (ConfigurationLimit, VelocityLimit)) or not any(limit is l for l in listed):
+            raise LimitDefinitionError(f"bounds apply to the ConfigurationLimit and VelocityLimit of the limits list, not "
+                                       f"{type(limit).__name__}" + (" (limits=None: the default ConfigurationLimit cannot be named)" if limits is None else ""))
+        idx = torch.as_tensor(np.array(limit.indices), device=q.device, dtype=torch.long)
+        if isinstance(limit, ConfigurationLimit):
+            for other in listed:
+                if other is not limit and isinstance(other, ConfigurationLimit) and np.intersect1d(other.indices, limit.indices).size:
+                    raise LimitDefinitionError("bounds of a ConfigurationLimit that shares dofs with another ConfigurationLimit of the list "
+                                               "are ambiguous: the device narrows every ConfigurationLimit of a dof")
+            if not isinstance(value, (tuple, list)) or len(value) != 2:
+                raise LimitDefinitionError("a ConfigurationLimit takes bounds (lower, upper), each None, [nq] or [B, nq]")
+            qadr = torch.as_tensor(np.asarray(flat.dof_qadr)[np.asarray(limit.indices)], device=q.device, dtype=torch.long)
+            if value[0] is not None:
+                lo = full(-np.inf) if lo is None else lo
+                lo[:, idx] = rows(value[0], nq, "lower bounds")[:, qadr]
+            if value[1] is not None:
+                up = full(np.inf) if up is None else up
+                up[:, idx] = rows(value[1], nq, "upper bounds")[:, qadr]
+        else:
+            vm = full(np.inf) if vm is None else vm
+            vm[:, idx] = torch.minimum(vm[:, idx], rows(value, len(limit.indices), "velocity caps"))
+    return lo, up, vm
+
+
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
              limits: Optional[Sequence[Limit]] = None) -> Problem:
     """QP of the IK problem (reference solve_ik.py:43-65): P = damping I + sum H_t, q = sum c_t,
@@ -160,7 +206,8 @@ def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, dam
 
 
 def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
-             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, posture_weights=None, **kwargs):
+             safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, posture_weights=None, bounds=None,
+             **kwargs):
     """Velocity v = dq / dt tangent to the configuration (reference solve_ik.py:68-105).
 
     `weights` maps a FrameTask / RelativeFrameTask to a [6] or [B, 6] array and a ComTask to a [3] or [B, 3] array of
@@ -171,16 +218,26 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     task's per-dof costs: instance b solves as if the task's cost had been set to cost * w[b] (PostureTask.set_cost).  A
     weight of 0 on every dof of a DampingTask solves that instance as if the task were not in the list.
 
+    `bounds` maps a ConfigurationLimit of `limits` to (lower, upper), each None, [nq] or [B, nq] indexed by qpos address like
+    ConfigurationLimit.lower / upper, and a VelocityLimit of `limits` to vmax, [k] or [B, k] in the order of its indices like
+    VelocityLimit.limit.  They narrow the limit's bounds per instance: instance b solves as if the limit had been built with
+    max(lower, lower[b]), min(upper, upper[b]) and min(vmax, vmax[b]) on the dofs it lists; other entries are not read.  The
+    values are final bounds (any min_distance_from_limits margin is the caller's to apply), they can only narrow, and a
+    ConfigurationLimit that shares dofs with another one of the list cannot be a key.  A cap of 0 keeps a dof where it is.
+    build_ik and compute_qp_inequalities still show the limits' own bounds.
+
     Returns a numpy (nv,) vector for a single configuration, a torch CUDA [B, nv] tensor for a batch.
     Raises NotWithinConfigurationLimits when `safety_break` and some instance is out of limits;
     raises AssertionError (like the reference's `assert dq is not None`) when the QP of any instance
     could not be solved.
     """
+    limits_arg = limits   # the caller's list: `bounds` keys name its limits
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
-    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, **kw)
+    bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
+    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, bounds=bd, **kw)
     st = status.cpu().numpy()
     if (st & 1).any():
         if safety_break:
@@ -196,7 +253,7 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
 
 def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
                 limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None):
+                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None, bounds=None):
     """The inner loop the reference's examples wrap around solve_ik (examples/arm_iiwa.py:63-70,
     examples/quadruped_spot.py:89-104), run on the device per instance:
 
@@ -210,13 +267,15 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path.
 
     `weights` as in solve_ik.  A frame task whose three position (orientation) weights are 0 in an instance is left out of
-    that instance's position (orientation) test.  `posture_weights` as in solve_ik."""
+    that instance's position (orientation) test.  `posture_weights` and `bounds` as in solve_ik."""
+    limits_arg = limits   # the caller's list: `bounds` keys name its limits
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
+    bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, **kw)
+                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, bounds=bd, **kw)
     configuration._sync_from_device()
     st = status.cpu().numpy()
     assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
@@ -228,7 +287,7 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None):
+             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None, bounds=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -254,6 +313,8 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
 
     `posture_weights` as in converge_ik, per frame: a PostureTask's or DampingTask's weights are a float, [nv] or [B, nv]
     (every frame), [T, nv] (shared by every instance) or [B, T, nv] (a 2-D array must then not leave B = T ambiguous).
+
+    `bounds` as in solve_ik, one value per instance that holds on every frame.
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
@@ -304,9 +365,11 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         posture = torch.stack([r.expand(lead, T, flat.nq) for r in rows], dim=2).contiguous()
         posture, posture_seq = (posture[0] if lead == 1 else posture), True
 
+    limits_arg = limits   # the caller's list: `bounds` keys name its limits
     prob, limits = _problem(configuration, tasks, limits)
     w = _task_weights(tasks, weights, q, T)
     pw = _posture_weights(tasks, posture_weights, q, flat.nv, T)
+    bd = _limit_bounds(limits_arg, bounds, q, flat)
     ln = None
     if lengths is not None:
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
@@ -315,7 +378,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
                                           ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq,
-                                          posture_weights=pw)
+                                          posture_weights=pw, bounds=bd)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran
