@@ -410,6 +410,55 @@ int bik_track_bounded64(const bik_problem* problem, int B, int T, double* q, con
                         int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
                         int32_t* status, int32_t* passes, void* stream);
 
+/* ---- per-instance collision avoidance ------------------------------------------------------------------------------------
+ * The ..._bounded entry points with one more argument, `coll`, right after `bounds`: each instance enables its own subset of
+ * the CollisionAvoidanceLimit's geom pairs and sets its own distances, as a mink user would build the limit with the pairs
+ * that matter now, or change minimum_distance_from_collisions / collision_detection_distance, between two solve_ik calls.
+ * With every candidate obstacle in the model, a pair mask gives each instance its own set of obstacles.
+ *   coll    host memory; its members are device buffers, each NULL for the problem's own: `enabled` [B][npairs] bytes
+ *           (bik_track_coll: [B][T][npairs]), `minimum_distance` and `detection_distance` [B] (bik_track_coll: [B][T]), float
+ *           or double like the other inputs (bik_inputs.f64).  bik_track_coll uses row b*T + t while instance b is on frame t.
+ *           A NULL `coll`, or one whose three members are NULL, runs exactly what the ..._bounded entry point runs, through
+ *           the same kernels, bit for bit.  A non-NULL member on a problem without a CollisionAvoidanceLimit: BIK_ERR_INVALID.
+ *   `weights`, `posture_weights` and `bounds` as in the ..._bounded entry points, each NULL for none.
+ *   Pair k of instance b is used iff enabled[b][k] != 0.  A disabled pair hands the QP what a pair beyond the detection
+ *   distance hands it (no constraint row), and its distance is never computed.  An instance with at least one enabled pair
+ *   gives, bit for bit, what a problem built with its enabled pairs (in the same order) and its distances gives: dq, q,
+ *   iterations and status.  One exception: the solver's iteration cap (60 + 2 (nv + min(npairs, 24))) counts the problem's
+ *   pairs, so an instance with fewer than 24 enabled pairs may iterate longer before BIK_STATUS_QP_MAXITER than that
+ *   problem would.  An instance with no enabled pair solves the QP without collision rows; it agrees with a problem built
+ *   without the limit to solver tolerance, not bit for bit (that problem may take fp32 kernels and another QP path).
+ *   The distances are used in the caller's precision where K1 runs in fp64, which it does for every problem with a
+ *   CollisionAvoidanceLimit unless BIK_K1_PRECISION=f32 is set.  A non-finite distance falls back to the problem's value and
+ *   sets BIK_STATUS_NONFINITE on the instance (bik_track_coll: on the frame in progress); no other value is refused.
+ *   The limit's gain and bound_relaxation stay the problem's, and bik_fk_jac, bik_solve, bik_limits_box and bik_step_host
+ *   have no collision form. */
+typedef struct bik_collision {
+  const uint8_t* enabled;          /* [B][npairs] (bik_track_coll: [B][T][npairs]) or NULL: pair k of instance b is used iff != 0 */
+  const void* minimum_distance;    /* [B] (track: [B][T]) or NULL: replaces minimum_distance_from_collisions */
+  const void* detection_distance;  /* [B] (track: [B][T]) or NULL: replaces collision_detection_distance */
+} bik_collision;                   /* distances: float or double like the other inputs (bik_inputs.f64) */
+int bik_step_coll(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                  const bik_bounds* bounds, const bik_collision* coll, float dt, double damping, int nsteps, int integrate, float* dq,
+                  int32_t* status, void* stream);
+int bik_converge_coll(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                      const bik_bounds* bounds, const bik_collision* coll, float dt, double damping, int max_iters, float pos_threshold,
+                      float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_coll(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                   const bik_bounds* bounds, const bik_collision* coll, const int32_t* lengths, float dt, double damping, int max_iters,
+                   float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
+                   int32_t* passes, void* stream);
+int bik_step_coll64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                    const bik_bounds* bounds, const bik_collision* coll, double dt, double damping, int nsteps, int integrate, double* dq,
+                    int32_t* status, void* stream);
+int bik_converge_coll64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                        const bik_bounds* bounds, const bik_collision* coll, double dt, double damping, int max_iters, double pos_threshold,
+                        double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_coll64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                     const void* posture_weights, const bik_bounds* bounds, const bik_collision* coll, const int32_t* lengths, double dt,
+                     double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj,
+                     int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */
 int bik_measure_fma_peak(int device, int use_double, int repeats, double* tflops);

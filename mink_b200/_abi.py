@@ -58,6 +58,10 @@ class BikBounds(C.Structure):   # per-instance bounds of the ..._bounded entry p
     _fields_ = [("lower", C.c_void_p), ("upper", C.c_void_p), ("vmax", C.c_void_p)]
 
 
+class BikCollision(C.Structure):   # per-instance collision pairs and distances of the ..._coll entry points: device buffers or NULL
+    _fields_ = [("enabled", C.c_void_p), ("minimum_distance", C.c_void_p), ("detection_distance", C.c_void_p)]
+
+
 class BikDims(C.Structure):
     _fields_ = [("nq", C.c_int32), ("nv", C.c_int32), ("nnode", C.c_int32), ("nframe", C.c_int32),
                 ("nposture", C.c_int32), ("ncom", C.c_int32), ("nrows", C.c_int32), ("npairs", C.c_int32)]

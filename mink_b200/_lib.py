@@ -5,7 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-from ._abi import BikBounds, BikDims, BikFrame, BikInputs, BikLimitDesc, BikTaskDesc
+from ._abi import BikBounds, BikCollision, BikDims, BikFrame, BikInputs, BikLimitDesc, BikTaskDesc
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libbik.so")
 _lib = None
@@ -19,7 +19,8 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_step_weighted", "bik_converge_weighted", "bik_track_weighted", "bik_step_weighted64", "bik_converge_weighted64",
            "bik_track_weighted64", "bik_step_weighted_ex", "bik_converge_weighted_ex", "bik_track_weighted_ex",
            "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64", "bik_step_bounded",
-           "bik_converge_bounded", "bik_track_bounded", "bik_step_bounded64", "bik_converge_bounded64", "bik_track_bounded64"]
+           "bik_converge_bounded", "bik_track_bounded", "bik_step_bounded64", "bik_converge_bounded64", "bik_track_bounded64",
+           "bik_step_coll", "bik_converge_coll", "bik_track_coll", "bik_step_coll64", "bik_converge_coll64", "bik_track_coll64"]
 
 
 class BikError(RuntimeError):
@@ -91,6 +92,9 @@ def load():
         # per-instance bounds: a bik_bounds after the posture weights
         getattr(lib, name.replace("64", "") + "_bounded" + ("64" if name.endswith("64") else "")).argtypes = (args[:at] + [vp, vp, C.POINTER(BikBounds)]
                                                                                                      + args[at:])
+        # per-instance collision pairs and distances: a bik_collision after the bounds
+        getattr(lib, name.replace("64", "") + "_coll" + ("64" if name.endswith("64") else "")).argtypes = (
+            args[:at] + [vp, vp, C.POINTER(BikBounds), C.POINTER(BikCollision)] + args[at:])
     _lib = lib
     return lib
 

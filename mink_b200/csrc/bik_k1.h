@@ -176,6 +176,38 @@ struct K1Args {
   // of b's frames K1 copies that frame's posture rows of ptgt into row b; K2 reads this buffer as its per-instance targets.
   void* ptcur;
 };
+// The arguments of the per-instance collision instantiation (k1c_kernel, k1_warp_tile<..., CO = true>): the ..._coll entry
+// points.  Row r of the buffers is instance b's (b*T + cursor[b] in track mode); each may be null.  enabled [rows][npairs]:
+// pair k is computed iff its byte is != 0, else it hands K2 what a pair beyond the detection distance hands it (a zero G row,
+// h = +inf) without its distance being computed.  dmin / ddet [rows], in the inputs' element type: the instance's
+// minimum_distance_from_collisions / collision_detection_distance; a non-finite value falls back to the problem's and sets
+// BIK_STATUS_NONFINITE on the instance.
+struct K1CArgs : K1Args {
+  const uint8_t* enabled;
+  const void* dmin;
+  const void* ddet;
+};
+// row of instance b in the K1CArgs buffers: b, or in track mode that of its current frame
+template <bool TR>
+BIK_HD long long k1c_row(const K1Args& a, int b) { return TR ? (long long)b * a.T + a.cursor[b] : (long long)b; }
+// row `row` of a distance buffer is finite (or the buffer is null)
+template <typename T>
+BIK_HD bool k1c_finite(const void* buf, long long row, int is64) {
+  if (!buf) return true;
+  const T v = ldin<T>(buf, row, is64);
+  return v - v == T(0);
+}
+// collision constant k of KC<T>::coll; CO: for k = 1 (minimum distance) and 2 (detection distance) the instance's value in row
+// `row` of the K1CArgs buffer instead, where the lane is valid and the buffer gives a finite one
+template <typename T, bool CO>
+BIK_HD T k1c_coll(const PView& P, const K1Args& a, bool valid, long long row, int k) {
+  if constexpr (CO) {
+    const K1CArgs& ca = static_cast<const K1CArgs&>(a);
+    const void* buf = k == 1 ? ca.dmin : (k == 2 ? ca.ddet : nullptr);
+    if (valid && buf && k1c_finite<T>(buf, row, a.in64)) return ldin<T>(buf, row, a.in64);
+  }
+  return KC<T>::coll(P, k);
+}
 // the thresholds of the convergence test in the instantiation's precision
 template <typename T>
 BIK_HD T k1_pos_thr(const K1Args& a) { if constexpr (sizeof(T) == 8) return a.pos_thr64; else return T(a.pos_thr); }
@@ -556,9 +588,11 @@ template <> BIK_HD void store6<double>(double* o, V3<double> top, V3<double> bot
 // PK (compile time): packed hand-off with the fused check_limits / convergence test (bik_step, bik_converge), else the dense
 // API form (bik_fk_jac) -- two instantiations so that neither carries the other's registers and code.
 // TR (compile time, with PK): track mode of bik_track (see K1Args); a third instantiation, so the other two are unchanged.
-template <typename T, int G, int W, bool PK, bool TR = false>
+// CO (compile time, with PK): `a` is a K1CArgs, per-instance collision pairs and distances (the ..._coll entry points).
+template <typename T, int G, int W, bool PK, bool TR = false, bool CO = false>
 BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int lane, K1Pipe* pipe = nullptr, int next_inst0 = -1) {
   static_assert(!TR || PK, "track mode writes the packed hand-off");
+  static_assert(!CO || PK, "per-instance collision pairs write the packed hand-off");
   const PHeader& h = P.h();
   constexpr int IPW = W / G;
   const int nv = h.nv, nq = h.nq, K = h.K;
@@ -566,6 +600,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
   const int b = inst0 + li;
   const int nvalid = (a.B - inst0) < IPW ? (a.B - inst0) : IPW;
   const bool valid = li < nvalid && (!TR || a.tstep[b] >= 0);   // track mode: an instance without frames left does no work
+  long long crow = 0;   // CO: the instance's row of the K1CArgs buffers, taken before track mode's test moves the cursor on
+  if constexpr (CO) crow = valid ? k1c_row<TR>(a, b) : 0;
   const int SS = k1_state_stride(h);
   constexpr bool packed = PK;
   const long long PKS = h.pk_stride;
@@ -654,6 +690,13 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         for (int k = lane; k < K; k += W) {
           const T w = ldin<T>(a.weights, w0 + k, a.in64);
           if (!(w >= T(0) && w <= T(1))) bad |= 32;
+        }
+      }
+      if constexpr (CO) {   // a non-finite collision distance: BIK_STATUS_NONFINITE (the problem's value is used)
+        const K1CArgs& ca = static_cast<const K1CArgs&>(a);
+        if (lane == 0) {
+          const long long r = k1c_row<TR>(a, inst0 + i);
+          if (!k1c_finite<T>(ca.dmin, r, a.in64) || !k1c_finite<T>(ca.ddet, r, a.in64)) bad |= 4;
         }
       }
       if (bad) {
@@ -981,7 +1024,14 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
     const int32_t* pairs = P.i(h.off_pairs);
     T* Gcg = reinterpret_cast<T*>(a.Gc);
     T* hcg = reinterpret_cast<T*>(a.hc);
-    const T ddet = KC<T>::coll(P, 2), dmin = KC<T>::coll(P, 1), cgain = KC<T>::coll(P, 0), relax = KC<T>::coll(P, 3);
+    // CO: the instance's distances (the problem's for a null buffer, a non-finite value or an invalid lane) and its row of the
+    // pair mask, or null (every pair)
+    const T ddet = k1c_coll<T, CO>(P, a, valid, crow, 2), dmin = k1c_coll<T, CO>(P, a, valid, crow, 1), cgain = KC<T>::coll(P, 0), relax = KC<T>::coll(P, 3);
+    const uint8_t* en = nullptr;
+    if constexpr (CO) {
+      const uint8_t* m = static_cast<const K1CArgs&>(a).enabled;
+      if (valid && m) en = m + crow * h.npairs;
+    }
     for (int p0 = 0; p0 < h.npairs; p0 += 6) {
       int np_ = h.npairs - p0 < 6 ? h.npairs - p0 : 6;
       zero_words<W, T>(stage, IPW * np_ * nv, lane);
@@ -990,7 +1040,7 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         for (int pi = g; pi < np_; pi += G) {
           const int i1 = pairs[2 * (p0 + pi)], i2 = pairs[2 * (p0 + pi) + 1];
           V3<T> o1, o2;
-          T dist = geom_distance<T>(P, i1, i2, xs, ddet, &o1, &o2);
+          T dist = !en || en[p0 + pi] ? geom_distance<T>(P, i1, i2, xs, ddet, &o1, &o2) : ddet;   // a disabled pair: as one beyond ddet
           T hval = T(BIK_INF_F);
           if (dist != ddet) {
             hval = dist > dmin ? cgain * (dist - dmin) / T(a.dt) + relax : relax;

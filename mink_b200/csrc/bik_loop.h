@@ -16,12 +16,15 @@ namespace bik {
 // fp64 (k1_auto_double, or io64).  dt and the thresholds of fp32 calls are their float values.  weights: the ..._weighted entry
 // points' per-instance task weights (K1Args::weights), or null.  posture_weights: the ..._weighted_ex entry points' per-instance
 // posture weights (K2PwArgs), or null.  bounds: the ..._bounded entry points' per-instance bounds (K2BdArgs), all three null
-// for none; held by value, so that the converge graph's key holds the three pointers.
+// for none; held by value, so that the converge graph's key holds the three pointers.  coll: the ..._coll entry points'
+// per-instance collision pairs and distances (K1CArgs), all three null for none; held by value for the same reason.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
   void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights; bik_bounds bounds;
+  bik_collision coll;
 };
 inline bool has_bounds(const bik_bounds& bd) { return bd.lower || bd.upper || bd.vmax; }
+inline bool has_coll(const bik_collision& co) { return co.enabled || co.minimum_distance || co.detection_distance; }
 
 // The loop state.  pk / Gc / hc: K1 -> K2 hand-off rows, fp64 when k1d.  dq: K2's dq of the previous pass (its warm start), in
 // the caller's precision.  warm: [B][max(nu,1)] active-set guess.  done: [B] K2 leaves the instance alone.  cursor / step /
@@ -61,6 +64,14 @@ inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status
     a.q_traj = c.q_traj; a.traj_status = status; a.warm = s.warm;
     if (posture_seq(in)) a.ptcur = s.ptcur;
   }
+  return a;
+}
+// The same for the collision instantiation of K1 (has_coll(c.coll)).  Track mode reads row b*T + cursor[b].
+inline K1CArgs conv_k1c_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  K1CArgs a;
+  memset(&a, 0, sizeof a);
+  static_cast<K1Args&>(a) = conv_k1_args(c, s, status);
+  a.enabled = c.coll.enabled; a.dmin = c.coll.minimum_distance; a.ddet = c.coll.detection_distance;
   return a;
 }
 // K2 of a pass: solves and integrates the instances K1 left undone, and does nothing once the condition said stop.

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._abi import POSTURE_SEQ_BATCHED, POSTURE_SEQ_SHARED, BikBounds, BikDims, BikInputs, ProblemSpec, c_frames
+from ._abi import POSTURE_SEQ_BATCHED, POSTURE_SEQ_SHARED, BikBounds, BikCollision, BikDims, BikInputs, ProblemSpec, c_frames
 from .flatten import FlatModel, Frame
 
 
@@ -208,6 +208,27 @@ class Problem:
             setattr(out, name, t.data_ptr())
         return out, keep
 
+    def _collision(self, collision, q: torch.Tensor, B: int, T: Optional[int] = None):
+        """Per-instance collision arguments (enabled, minimum_distance, detection_distance) as a BikCollision of contiguous CUDA
+        tensors, and the tensors it points to: enabled [B, npairs] (track: [B, T, npairs]) as uint8, the distances [B] (track:
+        [B, T]) in q's dtype.  None for None or three Nones (the call then runs the ..._bounded entry point)."""
+        if collision is None or all(x is None for x in collision):
+            return None, []
+        if len(collision) != 3:
+            raise ValueError("collision must be an (enabled, minimum_distance, detection_distance) tuple, each a tensor or None")
+        lead = (B,) if T is None else (B, T)
+        keep, out = [], BikCollision()
+        for name, x in zip(("enabled", "minimum_distance", "detection_distance"), collision):
+            if x is None:
+                continue
+            shape = lead + (self.npairs,) if name == "enabled" else lead
+            t = self.model._dev(x, dtype=torch.uint8 if name == "enabled" else q.dtype)
+            if tuple(t.shape) != shape:
+                raise ValueError(f"collision {name} must have shape {shape}, got {tuple(t.shape)}")
+            keep.append(t)
+            setattr(out, name, t.data_ptr())
+        return out, keep
+
     def fk_jac(self, q, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2):
         inp, keep, B, q = self._inputs(q, frame_targets, posture_targets, com_targets)
         dev, dt_ = q.device, q.dtype
@@ -257,27 +278,34 @@ class Problem:
 
     def step(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
              damping: float = 1e-12, nsteps: int = 1, integrate: bool = False, dq: Optional[torch.Tensor] = None,
-             status: Optional[torch.Tensor] = None, weights=None, posture_weights=None, bounds=None):
+             status: Optional[torch.Tensor] = None, weights=None, posture_weights=None, bounds=None, collision=None):
         """solve_ik (x nsteps, optionally integrating q in place).  q: [B,nq] fp32 or fp64 CUDA tensor.
         weights: [B, K] per-instance multipliers in [0, 1] of the frame / CoM task costs, rows in the stacked order of J
         (bik_step_weighted); None: the problem's costs.
         posture_weights: [B, P, nv] per-instance multipliers in [0, 1] of the PostureTask / DampingTask dof costs, tasks in the
         order of the posture targets (bik_step_weighted_ex); None: the problem's costs.
         bounds: (lower, upper, vmax), each [B, nv] (tangent dofs) or None, that narrow the problem's ConfigurationLimit bounds
-        and VelocityLimit caps per instance on the dofs those limits list (bik_step_bounded; bik.h); None: the problem's."""
+        and VelocityLimit caps per instance on the dofs those limits list (bik_step_bounded; bik.h); None: the problem's.
+        collision: (enabled, minimum_distance, detection_distance), each None or enabled [B, npairs] (pair k of instance b is
+        used iff != 0) and the distances [B], that replace the CollisionAvoidanceLimit's pairs and distances per instance
+        (bik_step_coll; bik.h); None: the problem's."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
         w = self._weights(weights, q, B)
         pw = self._posture_weights(posture_weights, q, B)
         bd, keep_bd = self._bounds(bounds, q, B)
+        co, keep_co = self._collision(collision, q, B)
         if dq is None:
             dq = torch.empty((B, self.nv), device=q.device, dtype=q.dtype)
         if status is None:
             status = torch.empty(B, device=q.device, dtype=torch.int32)
         assert dq.dtype == q.dtype
         args = (float(dt), float(damping), int(nsteps), int(bool(integrate)), dq.data_ptr(), status.data_ptr(), _stream())
-        if bd is not None:
+        if co is not None:
+            fn = self.lib.bik_step_coll64 if _is64(q) else self.lib.bik_step_coll
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
+        elif bd is not None:
             fn = self.lib.bik_step_bounded64 if _is64(q) else self.lib.bik_step_bounded
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), C.byref(bd), *args))
         elif pw is not None:
@@ -293,24 +321,28 @@ class Problem:
 
     def converge(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
                  damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-                 check_every: int = 1, weights=None, posture_weights=None, bounds=None):
+                 check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None):
         """solve_ik + integrate until every frame task is within the thresholds or max_iters steps were taken, per instance
         (the inner loop of the reference's examples; bik_converge for a float32 q, bik_converge64 for a float64 q, the
         targets in q's dtype).  q is updated in place.  weights: [B, K] as in `step` (bik_converge_weighted); a frame task
         whose three position (orientation) weights are 0 is left out of the position (orientation) test.
         posture_weights: [B, P, nv] as in `step` (bik_converge_weighted_ex).  bounds: as in `step` (bik_converge_bounded).
-        Returns (iters [B], status [B])."""
+        collision: as in `step` (bik_converge_coll).  Returns (iters [B], status [B])."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
         w = self._weights(weights, q, B)
         pw = self._posture_weights(posture_weights, q, B)
         bd, keep_bd = self._bounds(bounds, q, B)
+        co, keep_co = self._collision(collision, q, B)
         iters = torch.zeros(B, device=q.device, dtype=torch.int32)
         status = torch.zeros(B, device=q.device, dtype=torch.int32)
         args = (float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every), iters.data_ptr(),
                 status.data_ptr(), _stream())
-        if bd is not None:
+        if co is not None:
+            fn = self.lib.bik_converge_coll64 if _is64(q) else self.lib.bik_converge_coll
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
+        elif bd is not None:
             fn = self.lib.bik_converge_bounded64 if _is64(q) else self.lib.bik_converge_bounded
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), C.byref(bd), *args))
         elif pw is not None:
@@ -326,7 +358,7 @@ class Problem:
 
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-              check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None, bounds=None):
+              check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None, bounds=None, collision=None):
         """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
         bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
@@ -337,7 +369,9 @@ class Problem:
         passes is a 0-d tensor, the number of passes the device loop ran.
         weights: [B, T, K] per-frame task weights as in `converge` (bik_track_weighted), or None.
         posture_weights: [B, T, P, nv] per-frame posture weights as in `converge` (bik_track_weighted_ex), or None.
-        bounds: as in `converge`, [B, nv] each, one row per instance for every frame (bik_track_bounded), or None."""
+        bounds: as in `converge`, [B, nv] each, one row per instance for every frame (bik_track_bounded), or None.
+        collision: as in `converge` with one row per instance and frame, enabled [B, T, npairs] and the distances [B, T]
+        (bik_track_coll), or None."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         m = self.model
         B = q.shape[0]
@@ -358,6 +392,7 @@ class Problem:
         w = self._weights(weights, q, B, T)
         pw = self._posture_weights(posture_weights, q, B, T)
         bd, keep_bd = self._bounds(bounds, q, B)
+        co, keep_co = self._collision(collision, q, B, T)
         ln = None
         if lengths is not None:
             ln = m._dev(lengths, torch.int32).reshape(-1)
@@ -369,7 +404,10 @@ class Problem:
         passes = torch.zeros(1, device=q.device, dtype=torch.int32)
         args = (_ptr(ln), float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every),
                 q_traj.data_ptr(), iters.data_ptr(), status.data_ptr(), passes.data_ptr(), _stream())
-        if bd is not None:
+        if co is not None:
+            fn = self.lib.bik_track_coll64 if _is64(q) else self.lib.bik_track_coll
+            _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
+        elif bd is not None:
             fn = self.lib.bik_track_bounded64 if _is64(q) else self.lib.bik_track_bounded
             _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), C.byref(bd), *args))
         elif pw is not None:

@@ -15,7 +15,7 @@ import numpy as np
 from ._abi import ProblemSpec
 from .configuration import Configuration
 from .exceptions import InvalidTarget, LimitDefinitionError
-from .limits import ConfigurationLimit, Limit, VelocityLimit
+from .limits import CollisionAvoidanceLimit, ConfigurationLimit, Limit, VelocityLimit
 from .tasks import ComTask, DampingTask, FrameTask, PostureTask, Task, problem_for
 
 
@@ -181,6 +181,50 @@ def _limit_bounds(limits: Optional[Sequence[Limit]], bounds, q, flat):
     return lo, up, vm
 
 
+_COLLISION_KEYS = ("enabled", "minimum_distance_from_collisions", "collision_detection_distance")
+
+
+def _collision(limits: Optional[Sequence[Limit]], collision, q, T: Optional[int] = None):
+    """The (enabled, minimum_distance, detection_distance) buffers of a `collision={limit: {...}}` mapping, each None where the
+    dict leaves the key out; None for no mapping.  enabled: bools over limit.geom_id_pairs, [npairs] or [B, npairs], for a
+    sequence (T given) also [T, npairs] or [B, T, npairs]; the distances a float or [B], for a sequence also [T] or [B, T]."""
+    if not collision:
+        return None
+    import torch
+
+    listed = list(limits or [])
+    if len(collision) != 1:
+        raise LimitDefinitionError("collision takes one entry: the CollisionAvoidanceLimit of the limits list")
+    (limit, value), = collision.items()
+    if not isinstance(limit, CollisionAvoidanceLimit) or not any(limit is l for l in listed):
+        raise LimitDefinitionError(f"collision applies to the CollisionAvoidanceLimit of the limits list, not {type(limit).__name__}")
+    if not isinstance(value, dict) or not set(value) <= set(_COLLISION_KEYS):
+        raise LimitDefinitionError(f"collision values are dicts with the keys {', '.join(_COLLISION_KEYS)}, each optional")
+    B, npairs = q.shape[0], len(limit.geom_id_pairs)
+    lead = (B,) if T is None else (B, T)
+
+    def per_instance(x, tail, dtype, what):
+        x = x if isinstance(x, torch.Tensor) else torch.as_tensor(np.array(x))
+        x = x.to(device=q.device, dtype=dtype)
+        shapes = [tail, (B,) + tail] if T is None else [tail, (B,) + tail, (T,) + tail, (B, T) + tail]
+        if tuple(x.shape) not in shapes:
+            raise LimitDefinitionError(f"Expected {what} of shape {' or '.join(str(list(s)) for s in shapes)}, got {list(x.shape)}")
+        if T is not None and x.ndim == len(tail) + 1:
+            if B == T and B > 1:
+                raise LimitDefinitionError(f"{what} of shape {list(x.shape)} could be per instance or per frame (B = T = {B}): "
+                                           f"pass {list((B, T) + tail)}")
+            x = x.unsqueeze(1) if x.shape[0] == B else x.unsqueeze(0)
+        return x.expand(lead + tail).contiguous()
+
+    en = value.get("enabled")
+    dmin = value.get("minimum_distance_from_collisions")
+    ddet = value.get("collision_detection_distance")
+    return (None if en is None else per_instance(np.asarray(en, dtype=bool) if not isinstance(en, torch.Tensor) else en != 0,
+                                                 (npairs,), torch.uint8, "an enabled mask"),
+            None if dmin is None else per_instance(dmin, (), q.dtype, "minimum_distance_from_collisions"),
+            None if ddet is None else per_instance(ddet, (), q.dtype, "collision_detection_distance"))
+
+
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
              limits: Optional[Sequence[Limit]] = None) -> Problem:
     """QP of the IK problem (reference solve_ik.py:43-65): P = damping I + sum H_t, q = sum c_t,
@@ -207,7 +251,7 @@ def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, dam
 
 def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
              safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, posture_weights=None, bounds=None,
-             **kwargs):
+             collision=None, **kwargs):
     """Velocity v = dq / dt tangent to the configuration (reference solve_ik.py:68-105).
 
     `weights` maps a FrameTask / RelativeFrameTask to a [6] or [B, 6] array and a ComTask to a [3] or [B, 3] array of
@@ -226,18 +270,27 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     ConfigurationLimit that shares dofs with another one of the list cannot be a key.  A cap of 0 keeps a dof where it is.
     build_ik and compute_qp_inequalities still show the limits' own bounds.
 
+    `collision` maps the CollisionAvoidanceLimit of `limits` to a dict with any of the keys "enabled",
+    "minimum_distance_from_collisions" and "collision_detection_distance".  "enabled" is a bool array over the limit's
+    geom_id_pairs, [npairs] or [B, npairs]: instance b solves as if the limit had been built with its enabled pairs only
+    (limit.pair_mask(geoms) selects the pairs that involve some geoms).  The distances are a float or a [B] array that
+    replace the limit's attributes of those names per instance; a non-finite distance keeps the limit's own and flags the
+    instance.  compute_qp_inequalities still shows the limit's own pairs and distances.
+
     Returns a numpy (nv,) vector for a single configuration, a torch CUDA [B, nv] tensor for a batch.
     Raises NotWithinConfigurationLimits when `safety_break` and some instance is out of limits;
     raises AssertionError (like the reference's `assert dq is not None`) when the QP of any instance
     could not be solved.
     """
-    limits_arg = limits   # the caller's list: `bounds` keys name its limits
+    limits_arg = limits   # the caller's list: `bounds` and `collision` keys name its limits
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
     bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
-    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, bounds=bd, **kw)
+    co = _collision(limits_arg, collision, q)
+    dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, bounds=bd, collision=co,
+                           **kw)
     st = status.cpu().numpy()
     if (st & 1).any():
         if safety_break:
@@ -253,7 +306,7 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
 
 def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
                 limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None, bounds=None):
+                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None):
     """The inner loop the reference's examples wrap around solve_ik (examples/arm_iiwa.py:63-70,
     examples/quadruped_spot.py:89-104), run on the device per instance:
 
@@ -267,15 +320,17 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path.
 
     `weights` as in solve_ik.  A frame task whose three position (orientation) weights are 0 in an instance is left out of
-    that instance's position (orientation) test.  `posture_weights` and `bounds` as in solve_ik."""
-    limits_arg = limits   # the caller's list: `bounds` keys name its limits
+    that instance's position (orientation) test.  `posture_weights`, `bounds` and `collision` as in solve_ik."""
+    limits_arg = limits   # the caller's list: `bounds` and `collision` keys name its limits
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
     w = _task_weights(tasks, weights, q)
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
     bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
+    co = _collision(limits_arg, collision, q)
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
-                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, bounds=bd, **kw)
+                                  ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, bounds=bd,
+                                  collision=co, **kw)
     configuration._sync_from_device()
     st = status.cpu().numpy()
     assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
@@ -287,7 +342,8 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None, bounds=None):
+             ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None, bounds=None,
+             collision=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -315,6 +371,10 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     (every frame), [T, nv] (shared by every instance) or [B, T, nv] (a 2-D array must then not leave B = T ambiguous).
 
     `bounds` as in solve_ik, one value per instance that holds on every frame.
+
+    `collision` as in solve_ik, per frame: "enabled" is [npairs] or [B, npairs] (every frame), [T, npairs] (shared by every
+    instance) or [B, T, npairs]; a distance is a float or [B] (every frame), [T] or [B, T] (a 2-D mask or a 1-D distance must
+    then not leave B = T ambiguous).
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
@@ -365,11 +425,12 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         posture = torch.stack([r.expand(lead, T, flat.nq) for r in rows], dim=2).contiguous()
         posture, posture_seq = (posture[0] if lead == 1 else posture), True
 
-    limits_arg = limits   # the caller's list: `bounds` keys name its limits
+    limits_arg = limits   # the caller's list: `bounds` and `collision` keys name its limits
     prob, limits = _problem(configuration, tasks, limits)
     w = _task_weights(tasks, weights, q, T)
     pw = _posture_weights(tasks, posture_weights, q, flat.nv, T)
     bd = _limit_bounds(limits_arg, bounds, q, flat)
+    co = _collision(limits_arg, collision, q, T)
     ln = None
     if lengths is not None:
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
@@ -378,7 +439,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
                                           ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq,
-                                          posture_weights=pw, bounds=bd)
+                                          posture_weights=pw, bounds=bd, collision=co)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran

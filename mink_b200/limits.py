@@ -182,6 +182,20 @@ class CollisionAvoidanceLimit(Limit):
                 out.append((min(a, b), max(a, b)))
         return out
 
+    def pair_mask(self, geoms) -> np.ndarray:
+        """[len(geom_id_pairs)] bools: True for the pairs that involve any of `geoms` (names or ids).  For the per-instance
+        `enabled` mask of solve_ik / converge_ik / track_ik's `collision` argument: ~limit.pair_mask(["wall"]) drops the wall."""
+        names = self._flat.names["geom"]
+        ids = set()
+        for g in geoms:
+            if isinstance(g, str):
+                if g not in names:
+                    raise LimitDefinitionError(f"pair_mask: no geom named {g!r}")
+                ids.add(names.index(g))
+            else:
+                ids.add(int(g))
+        return np.array([a in ids or b in ids for a, b in self.geom_id_pairs], dtype=bool)
+
     def _spec(self, flat):
         used = sorted({g for p in self.geom_id_pairs for g in p})
         local = {g: i for i, g in enumerate(used)}
