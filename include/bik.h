@@ -459,6 +459,35 @@ int bik_track_coll64(const bik_problem* problem, int B, int T, double* q, const 
                      double damping, int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj,
                      int32_t* iters, int32_t* status, int32_t* passes, void* stream);
 
+/* ---- held targets in bik_track ------------------------------------------------------------------------------------------
+ * bik_track_coll with one more argument, `hold`, right after `coll`: a task can hold the value it had at the configuration
+ * the solver reached, for a run of frames, as a mink loop that calls task.set_target_from_configuration(configuration) before
+ * the first frame of the run does.  Contact locking is the typical use: a foot that touches down on frame t0 keeps the pose
+ * the robot's foot had when frame t0 began, for as long as the contact lasts.
+ *   hold    device, [B][T][H] bytes or NULL, H = F + C + P: the F frame-like tasks (FRAME and RELATIVE_FRAME) in the order of
+ *           frame_targets, then the C CoM tasks in the order of com_targets, then the P posture-type tasks in the order of
+ *           posture_targets.  A NULL `hold` runs exactly what bik_track_coll runs, through the same kernels, bit for bit.
+ *   `weights`, `posture_weights`, `bounds`, `coll` and `lengths` as in bik_track_coll.
+ *   A run of task k for instance b is a maximal set of consecutive frames t0..t1 with hold[b][t][k] != 0.  On the first pass
+ *   of frame t0, before that pass's errors are computed, the task's value at the instance's configuration (q_traj[b][t0-1],
+ *   or the start q for t0 = 0) is captured: a FRAME task's world pose as bik_fk reports it, a RELATIVE_FRAME task's pose in
+ *   its root (root^-1 * frame), a CoM task's CoM, a posture-type task's q.  It is stored in the caller's precision
+ *   (bik_inputs.f64), as a target the caller passed would be, and is the task's target on every frame of the run in place of
+ *   its row of frame_targets / com_targets / posture_targets; it is not captured again within the run.  Frames outside runs
+ *   read their targets as bik_track_coll does.  So each instance gives what T bik_converge_coll calls give when the caller
+ *   sets each held task's target with set_target_from_configuration before the first frame of each of its runs.  The
+ *   convergence test takes a held frame task's error against the held target, and weights apply to held tasks unchanged.
+ *   A hold on a posture-type task with gain 0 (a DampingTask) changes nothing.  An all-zero mask gives what bik_track_coll
+ *   gives: q_traj, iters, status and passes. */
+int bik_track_hold(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                   const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold, const int32_t* lengths, float dt, double damping,
+                   int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
+                   int32_t* passes, void* stream);
+int bik_track_hold64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                     const void* posture_weights, const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold,
+                     const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
+                     int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */
 int bik_measure_fma_peak(int device, int use_double, int repeats, double* tflops);

@@ -20,7 +20,8 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_track_weighted64", "bik_step_weighted_ex", "bik_converge_weighted_ex", "bik_track_weighted_ex",
            "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64", "bik_step_bounded",
            "bik_converge_bounded", "bik_track_bounded", "bik_step_bounded64", "bik_converge_bounded64", "bik_track_bounded64",
-           "bik_step_coll", "bik_converge_coll", "bik_track_coll", "bik_step_coll64", "bik_converge_coll64", "bik_track_coll64"]
+           "bik_step_coll", "bik_converge_coll", "bik_track_coll", "bik_step_coll64", "bik_converge_coll64", "bik_track_coll64",
+           "bik_track_hold", "bik_track_hold64"]
 
 
 class BikError(RuntimeError):
@@ -95,6 +96,11 @@ def load():
         # per-instance collision pairs and distances: a bik_collision after the bounds
         getattr(lib, name.replace("64", "") + "_coll" + ("64" if name.endswith("64") else "")).argtypes = (
             args[:at] + [vp, vp, C.POINTER(BikBounds), C.POINTER(BikCollision)] + args[at:])
+    # held targets (bik_track only): the hold mask after the collision arguments
+    for name in ("bik_track_coll", "bik_track_coll64"):
+        args = getattr(lib, name).argtypes
+        at = args.index(C.POINTER(BikCollision)) + 1
+        getattr(lib, name.replace("_coll", "_hold")).argtypes = args[:at] + [vp] + args[at:]
     _lib = lib
     return lib
 

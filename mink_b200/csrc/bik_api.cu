@@ -457,11 +457,12 @@ int Handoff::reserve(const PHeader& h, size_t B, int elem, unsigned* moves) {
   CUDA_OK(warm.reserve(B * n.warm, moves));
   return BIK_OK;
 }
-int LoopState::reserve(const PHeader& h, size_t B, int elem, bool ptseq, unsigned* moves) {
+int LoopState::reserve(const PHeader& h, size_t B, int elem, bool ptc, bool hold, unsigned* moves) {
   for (DevBuf* b : {&done, &cursor, &step, &status}) CUDA_OK(b->reserve(sizeof(int32_t) * B, moves));
   CUDA_OK(dq.reserve(elem * B * h.nv, moves));
   CUDA_OK(count.reserve(4 * sizeof(int), moves));
-  if (ptseq) CUDA_OK(ptcur.reserve(elem * B * (size_t)(h.P > 0 ? h.P : 1) * h.nq, moves));
+  if (ptc) CUDA_OK(ptcur.reserve(elem * B * (size_t)(h.P > 0 ? h.P : 1) * h.nq, moves));
+  if (hold) CUDA_OK(held.reserve(elem * B * (size_t)(k1_tgt_words(h) > 0 ? k1_tgt_words(h) : 1), moves));
   if (!host) CUDA_OK(cudaMallocHost(&host, 4 * sizeof(int)));
   return BIK_OK;
 }
@@ -636,13 +637,14 @@ static ConvBufs conv_bufs(const bik_problem* p) {
   const Handoff& w = p->hand;
   const LoopState& l = p->loop;
   return ConvBufs{w.pk.ptr, w.Gc.ptr, w.hc.ptr, l.dq.ptr, w.warm.as<signed char>(), l.done.as<int32_t>(), l.cursor.as<int32_t>(), l.step.as<int32_t>(),
-                  l.status.as<int32_t>(), l.count.as<int>(), l.ptcur.ptr};
+                  l.status.as<int32_t>(), l.count.as<int>(), l.ptcur.ptr, l.held.ptr};
 }
 // `status` is the call's status buffer, or null (the warm-up pass before a graph capture)
 static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
   const ConvBufs s = conv_bufs(p);
   conv_tick_kernel<<<1, 1, 0, st>>>(c.track, s.count);
-  int rc = has_coll(c.coll) ? bik_launch_k1(p, conv_k1c_args(c, s, status), c.k1d, st) : bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st);
+  int rc = c.hold ? bik_launch_k1(p, conv_k1h_args(c, s, status), c.k1d, st)
+                  : (has_coll(c.coll) ? bik_launch_k1(p, conv_k1c_args(c, s, status), c.k1d, st) : bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st));
   if (rc) return rc;
   conv_cond_kernel<<<1, 1, 0, st>>>(c.track, c.max_iters, s.count, handle, use_handle);
   if (has_bounds(c.bounds)) rc = dispatch_k2(p, conv_k2_bd_args(c, s, status), st);
@@ -721,7 +723,7 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   DeviceGuard g(p->model->device);
   int rc = p->hand.reserve(p->h, c.B, c.k1d ? 8 : 4, &p->moves);
   if (rc) return rc;
-  rc = p->loop.reserve(p->h, c.B, c.io64 ? 8 : 4, posture_seq(c.in), &p->moves);   // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
+  rc = p->loop.reserve(p->h, c.B, c.io64 ? 8 : 4, uses_ptcur(c), c.hold != nullptr, &p->moves);   // K2 writes dq in the caller's precision and reads it back as the next pass's warm start
   if (rc) return rc;
   rc = ws_acquire(p, st);
   if (rc) return rc;
@@ -823,9 +825,11 @@ extern "C" int bik_converge_coll64(const bik_problem* cp, int B, double* q, cons
 // The examples' outer loop: for each frame of a target sequence, the bik_converge loop, every instance on its own cursor.
 // One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
 // moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
+// hold: the bik_track_hold entry points' hold mask, or null.
 static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                         const bik_bounds* bounds, const bik_collision* coll, const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
-                        double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status, int32_t* passes, int io64, void* stream) {
+                        double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status, int32_t* passes, int io64, void* stream,
+                        const uint8_t* hold = nullptr) {
   if (B == 0 && cp) return BIK_OK;
   bounds = bounds_of(bounds);
   coll = coll_of(coll);
@@ -851,6 +855,7 @@ static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_
   c.k1d = k1_double(p, damping, io64 != 0, posture_weights != nullptr); c.io64 = io64 != 0; c.weights = weights; c.posture_weights = posture_weights;
   if (bounds) c.bounds = *bounds;
   if (coll) c.coll = *coll;
+  c.hold = hold;
   return converge_run(p, c, check_every, passes, st);
 }
 extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
@@ -911,6 +916,20 @@ extern "C" int bik_track_coll64(const bik_problem* cp, int B, int T, double* q, 
                                 int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
   return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
                       iters, status, passes, 1, stream);
+}
+extern "C" int bik_track_hold(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                              const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold, const int32_t* lengths, float dt, double damping,
+                              int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj, int32_t* iters, int32_t* status,
+                              int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 0, stream, hold);
+}
+extern "C" int bik_track_hold64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                                const void* posture_weights, const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold,
+                                const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
+                                int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 1, stream, hold);
 }
 extern "C" int bik_track64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
                            int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,

@@ -131,11 +131,12 @@ struct LoopState {
   DevBuf dq;                   // [B][nv] K2's dq of the previous pass (its warm start), 4- or 8-byte elements by the caller's precision
   DevBuf cursor, step, status; // [B] each: bik_track's frame cursor, steps taken in that frame, status of the frame in progress
   DevBuf count;                // device: { steps taken so far, unconverged instances, go }
-  DevBuf ptcur;                // [B][P][nq] bik_track's posture targets of each instance's current frame (sequence calls only)
+  DevBuf ptcur;                // [B][P][nq] bik_track's posture targets of each instance's current frame (bik_loop.h: uses_ptcur)
+  DevBuf held;                 // [B][7F + 3C] bik_track_hold's held frame and CoM targets (calls with a hold mask only)
   int* host = nullptr;         // pinned mirror of count
   ConvGraph graph;
-  // elem: bytes of the caller's elements; ptseq: the call has a posture target sequence
-  int reserve(const bik::PHeader& h, size_t B, int elem, bool ptseq, unsigned* moves);
+  // elem: bytes of the caller's elements; ptcur: the call keeps posture targets in ptcur; hold: the call has a hold mask
+  int reserve(const bik::PHeader& h, size_t B, int elem, bool ptcur, bool hold, unsigned* moves);
   ~LoopState() { graph.drop(); if (host) cudaFreeHost(host); }
 };
 
@@ -180,6 +181,7 @@ int bik_launch_geometry(const void* kern, const bik_model* m, size_t smem, int t
 // launchers (each returns BIK_OK or records an error)
 int bik_launch_k1(const bik_problem* p, const bik::K1Args& a, bool use_double, cudaStream_t st);
 int bik_launch_k1(const bik_problem* p, const bik::K1CArgs& a, bool use_double, cudaStream_t st);   // per-instance collision pairs (k1c_kernel)
+int bik_launch_k1(const bik_problem* p, const bik::K1HArgs& a, bool use_double, cudaStream_t st);   // held targets (k1h_kernel)
 int bik_launch_fk(const bik_model* m, const bik::FkArgs& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2Args& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2PwArgs& a, cudaStream_t st);   // posture-weighted instantiations

@@ -83,6 +83,44 @@ __global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1
   }
 }
 
+// Track mode with held targets (K1HArgs): the bik_track_hold entry points, with (CO) or without per-instance collision
+// arguments.  A kernel of its own for the same reason.
+template <typename T, int G, bool CO>
+__global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1h_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K1HArgs a) {
+  constexpr bool PK = true;
+  extern __shared__ __align__(16) uint32_t smem[];
+  __shared__ __align__(8) uint64_t bar;
+  __shared__ __align__(8) uint64_t pbar[4];   // one input-pipeline barrier per warp
+  stage_image(smem, gimage, words, &bar, use_tma);
+  PView P{smem};
+  const PHeader& h = P.h();
+  constexpr int IPW = 32 / G;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  T* wsm = reinterpret_cast<T*>(smem + words) + (size_t)warp * k1_warp_words(h, IPW);
+  const int ntiles = (a.B + IPW - 1) / IPW, stride = gridDim.x * nwarps;
+  int tile = blockIdx.x * nwarps + warp;
+  // Input pipeline: tile t computes its Jacobian columns while the q rows and targets of tile t + stride arrive by bulk async
+  // copy (BIK_USE_TMA=0 turns it off together with the staged image: plain loads at the top of every tile).
+  K1Pipe pipe{&pbar[warp], 0u, -1};
+  K1Pipe* pp = use_tma ? &pipe : nullptr;
+  if (pp) {
+    if (lane == 0) {
+      mbar_init(pipe.bar, 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    if (tile < ntiles && k1_tile_bulk_ok<T, true>(h, a, tile * IPW, IPW)) {
+      T* qtile = wsm + k1_qtile_offset(h, IPW);
+      if (lane == 0) k1_pipe_arm<T, true>(h, a, tile * IPW, IPW, &pipe, qtile, qtile + ((IPW * h.nq + 3) & ~3));
+      pipe.armed = tile * IPW;
+    }
+  }
+  for (; tile < ntiles; tile += stride) {
+    const int next = tile + stride < ntiles ? (tile + stride) * IPW : -1;
+    k1_warp_tile<T, G, 32, PK, true, CO, true>(P, a, tile * IPW, wsm, lane, pp, next);
+  }
+}
+
 template <typename T, int G>
 __global__ void __launch_bounds__(128) fk_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, FkArgs a) {
   extern __shared__ __align__(16) uint32_t smem[];
@@ -96,11 +134,9 @@ __global__ void __launch_bounds__(128) fk_kernel(const uint32_t* __restrict__ gi
   for (int tile = blockIdx.x * nwarps + warp; tile < ntiles; tile += gridDim.x * nwarps) fk_warp_tile<T, G, 32>(P, a, tile * IPW, wsm, lane);
 }
 
-// A: K1Args (k1_kernel<T, G, PK, TR>) or K1CArgs (k1c_kernel<T, G, TR>, PK)
-template <typename T, int G, bool PK, bool TR, typename A = K1Args>
-static int launch_k1_pk(const bik_problem* p, const A& a, cudaStream_t st) {
-  constexpr bool CO = std::is_same<A, K1CArgs>::value;
-  static_assert(!CO || PK, "k1c_kernel writes the packed hand-off");
+// Launch K1 kernel `kern` (a k1_kernel, k1c_kernel or k1h_kernel instantiation of scalar type T and G lanes per instance).
+template <typename T, int G, typename A>
+static int launch_k1_kernel(const bik_problem* p, void (*kern)(const uint32_t*, int, int, A), const A& a, cudaStream_t st) {
   const PHeader& h = p->h;
   constexpr int IPW = 32 / G;
   const int words = sizeof(T) == 8 ? h.words64 : h.words32;   // the fp64 side tables only travel with the fp64 instantiation
@@ -110,22 +146,25 @@ static int launch_k1_pk(const bik_problem* p, const A& a, cudaStream_t st) {
   size_t smem = need(NW);
   int grid = 1;
   long long tiles = ((long long)a.B + IPW - 1) / IPW;
-  const void* kern = CO ? (const void*)k1c_kernel<T, G, TR> : (const void*)k1_kernel<T, G, PK, TR>;
-  int rc = bik_launch_geometry(kern, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
+  int rc = bik_launch_geometry((const void*)kern, p->model, smem, 32 * NW, (tiles + NW - 1) / NW, &grid);
   if (rc) return rc;
-  if constexpr (CO) k1c_kernel<T, G, TR><<<grid, 32 * NW, smem, st>>>(p->d_image, words, p->model->use_tma, a);
-  else k1_kernel<T, G, PK, TR><<<grid, 32 * NW, smem, st>>>(p->d_image, words, p->model->use_tma, a);
+  kern<<<grid, 32 * NW, smem, st>>>(p->d_image, words, p->model->use_tma, a);
   CUDA_OK(cudaGetLastError());
   return BIK_OK;
 }
 template <typename T, int G>
 static int launch_k1(const bik_problem* p, const K1Args& a, cudaStream_t st) {
-  if (!a.pk) return launch_k1_pk<T, G, false, false>(p, a, st);
-  return a.cursor ? launch_k1_pk<T, G, true, true>(p, a, st) : launch_k1_pk<T, G, true, false>(p, a, st);
+  if (!a.pk) return launch_k1_kernel<T, G>(p, k1_kernel<T, G, false, false>, a, st);
+  return launch_k1_kernel<T, G>(p, a.cursor ? k1_kernel<T, G, true, true> : k1_kernel<T, G, true, false>, a, st);
 }
 template <typename T, int G>
 static int launch_k1(const bik_problem* p, const K1CArgs& a, cudaStream_t st) {
-  return a.cursor ? launch_k1_pk<T, G, true, true>(p, a, st) : launch_k1_pk<T, G, true, false>(p, a, st);
+  return launch_k1_kernel<T, G>(p, a.cursor ? k1c_kernel<T, G, true> : k1c_kernel<T, G, false>, a, st);
+}
+template <typename T, int G>
+static int launch_k1(const bik_problem* p, const K1HArgs& a, cudaStream_t st) {
+  const bool co = a.enabled || a.dmin || a.ddet;
+  return launch_k1_kernel<T, G>(p, co ? k1h_kernel<T, G, true> : k1h_kernel<T, G, false>, a, st);
 }
 template <typename T, typename A>
 static int dispatch_k1(const bik_problem* p, const A& a, cudaStream_t st) {
@@ -145,6 +184,11 @@ int bik_launch_k1(const bik_problem* p, const K1Args& a, bool use_double, cudaSt
 int bik_launch_k1(const bik_problem* p, const K1CArgs& a, bool use_double, cudaStream_t st) {
   if (!use_double && a.in64) return bik_fail(BIK_ERR_INVALID, "fp64 inputs need the fp64 instantiation of K1");
   if (!a.pk) return bik_fail(BIK_ERR_INVALID, "per-instance collision pairs need the packed hand-off");
+  return use_double ? dispatch_k1<double>(p, a, st) : dispatch_k1<float>(p, a, st);
+}
+int bik_launch_k1(const bik_problem* p, const K1HArgs& a, bool use_double, cudaStream_t st) {
+  if (!use_double && a.in64) return bik_fail(BIK_ERR_INVALID, "fp64 inputs need the fp64 instantiation of K1");
+  if (!a.pk || !a.cursor || !a.held) return bik_fail(BIK_ERR_INVALID, "held targets need track mode's packed hand-off and a held buffer");
   return use_double ? dispatch_k1<double>(p, a, st) : dispatch_k1<float>(p, a, st);
 }
 

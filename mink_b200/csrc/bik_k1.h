@@ -187,6 +187,27 @@ struct K1CArgs : K1Args {
   const void* dmin;
   const void* ddet;
 };
+// The arguments of the held-target instantiation (k1h_kernel, k1_warp_tile<..., TR, CO, HO = true>): the bik_track_hold entry
+// points, track mode only; the collision members as in K1CArgs, each may be null.  hold [B][T][H], H = F + C + P: byte k of
+// row b*T + t is != 0 iff instance b holds task k on frame t (frame-like tasks, then CoM tasks, then posture-type tasks, each
+// in the order of its target buffer).  On the first pass of the frame a run of held frames starts on, K1 captures the task's
+// value at q in the caller's precision: into held ([B][7F + 3C], frame tasks then CoM tasks) for frame and CoM tasks, into b's
+// row of ptcur for posture-type tasks.  Every pass of the run then takes that value as the task's target.  ptcur is set, and
+// filled from ptgt on the first pass of every frame that does not hold the task, whatever pbatched says.
+struct K1HArgs : K1CArgs {
+  const uint8_t* hold;
+  void* held;
+};
+// Task k of instance b on its current frame: 0 not held, 1 held (the target is the held value), 2 held and its run starts on
+// this frame, whose first pass this is (capture the value now).  Read before track mode's test moves the cursor on.
+BIK_HD int k1h_hold(const K1Args& a, const PHeader& h, int b, int k) {
+  const uint8_t* hold = static_cast<const K1HArgs&>(a).hold;
+  const long long H = h.F + h.C + h.P, row = (long long)b * a.T + a.cursor[b];
+  if (!hold[row * H + k]) return 0;
+  return a.tstep[b] == 0 && (a.cursor[b] == 0 || !hold[(row - 1) * H + k]) ? 2 : 1;
+}
+// v as the caller's precision holds it (a captured target is stored there, as a target the caller passed would be)
+template <typename T> BIK_HD T k1h_round(T v, int is64) { return sizeof(T) == 8 && !is64 ? T(float(v)) : v; }
 // row of instance b in the K1CArgs buffers: b, or in track mode that of its current frame
 template <bool TR>
 BIK_HD long long k1c_row(const K1Args& a, int b) { return TR ? (long long)b * a.T + a.cursor[b] : (long long)b; }
@@ -348,6 +369,35 @@ BIK_HD void frame_pose(int node, V3<T> lpos, Q4<T> lquat, const T* xs, Q4<T>* qf
   Q4<T> nq = ld_q(xs + 7 * node);
   *qf = qnormalize(qmul(nq, lquat));
   *pf = ld_v(xs + 7 * node + 4) + qrot(nq, lpos);
+}
+// root^-1 * frame for two world poses as bik_fk reports them, composed as mink's SE3 does (root.inverse() @ frame): the pose a
+// held RELATIVE_FRAME task captures (RelativeFrameTask.set_target_from_configuration)
+template <typename T>
+BIK_HD void held_relative(Q4<T> qr, V3<T> pr, Q4<T> qf, V3<T> pf, Q4<T>* q, V3<T>* p) {
+  const Q4<T> r = qconj(qr);
+  *q = qmul(r, qf);
+  *p = qrot(r, pf) - qrot(r, pr);
+}
+// The pose a held frame task captures from the frame's world pose (qf, pf) and, for a RELATIVE_FRAME, its root's (qr, pr), as
+// frame_pose gives them: the world pose as bik_fk reports it (FrameTask.set_target_from_configuration), or held_relative.
+template <typename T>
+BIK_HD void held_frame_value(bool relative, Q4<T> qf, V3<T> pf, Q4<T> qr, V3<T> pr, Q4<T>* q, V3<T>* p) {
+  *q = mat2quat(q2mat(qf)); *p = pf;
+  if (relative) held_relative<T>(mat2quat(q2mat(qr)), pr, *q, pf, q, p);
+}
+// The model's CoM at the node poses xs (mj_comPos's subtree_com of body 1), summed as bik_fk sums it (fk_warp_tile), over the
+// nodes with mass below them: K1 does not pose the others, whose terms in bik_fk's sum are exact zeros.
+template <typename T>
+BIK_HD V3<T> model_com(const PView& P, const T* xs) {
+  const PHeader& h = P.h();
+  V3<T> tot = KC<T>::com_fixed(P);
+  for (int n = 0; n < h.nnode; ++n) {
+    if (!(KC<T>::sub_m(P, n) > T(0))) continue;
+    tot = tot + KC<T>::own_m(P, n) * ld_v(xs + 7 * n + 4) + qrot(ld_q(xs + 7 * n), KC<T>::own_c(P, n));
+  }
+  T M = KC<T>::com_mass(P);
+  T invM = M > T(0) ? T(1) / M : T(0);
+  return v3<T>(tot.x * invM, tot.y * invM, tot.z * invM);
 }
 
 // World-aligned point-Jacobian column of dof `d` (owned by node n) for a point p moving with a
@@ -589,10 +639,12 @@ template <> BIK_HD void store6<double>(double* o, V3<double> top, V3<double> bot
 // API form (bik_fk_jac) -- two instantiations so that neither carries the other's registers and code.
 // TR (compile time, with PK): track mode of bik_track (see K1Args); a third instantiation, so the other two are unchanged.
 // CO (compile time, with PK): `a` is a K1CArgs, per-instance collision pairs and distances (the ..._coll entry points).
-template <typename T, int G, int W, bool PK, bool TR = false, bool CO = false>
+// HO (compile time, with TR): `a` is a K1HArgs, held targets (the bik_track_hold entry points).
+template <typename T, int G, int W, bool PK, bool TR = false, bool CO = false, bool HO = false>
 BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int lane, K1Pipe* pipe = nullptr, int next_inst0 = -1) {
   static_assert(!TR || PK, "track mode writes the packed hand-off");
   static_assert(!CO || PK, "per-instance collision pairs write the packed hand-off");
+  static_assert(!HO || TR, "held targets are a track-mode feature");
   const PHeader& h = P.h();
   constexpr int IPW = W / G;
   const int nv = h.nv, nq = h.nq, K = h.K;
@@ -644,7 +696,27 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         for (int k = lane; k < CW; k += W) ttile[IPW * FW + i * CW + k] = ldin<T>(a.ctgt, row * CW + k, a.in64);
       }
     }
-    if constexpr (TR) {   // first pass of a frame: its posture rows become the instance's row of ptcur, which this pass's K2 reads
+    if constexpr (HO) {   // first pass of a frame: each posture-type task's row of ptcur, which this pass's K2 reads
+      const int PW = h.P * nq;
+      for (int i = 0; i < nvalid; ++i) {
+        const int bi = inst0 + i;
+        if (a.tstep[bi] != 0) continue;
+        const long long r0 = a.pbatched == 3 ? (long long)bi * a.T + a.cursor[bi] : (a.pbatched == 2 ? a.cursor[bi] : (a.pbatched == 1 ? bi : 0));
+        for (int p = 0; p < h.P; ++p) {
+          const int s = k1h_hold(a, h, bi, h.F + h.C + p);
+          if (s == 1) continue;   // held since an earlier frame: the captured q stays
+          // the run starts here: q itself; not held: the frame's row of the posture targets
+          const void* src = s == 2 ? a.q : a.ptgt;
+          const long long so = s == 2 ? (long long)bi * nq : (r0 * h.P + p) * nq, dst = (long long)bi * PW + (long long)p * nq;
+          if constexpr (sizeof(T) == 8) {
+            if (a.in64)
+              for (int k = lane; k < nq; k += W) static_cast<double*>(a.ptcur)[dst + k] = static_cast<const double*>(src)[so + k];
+          }
+          if (sizeof(T) == 4 || !a.in64)
+            for (int k = lane; k < nq; k += W) static_cast<float*>(a.ptcur)[dst + k] = static_cast<const float*>(src)[so + k];
+        }
+      }
+    } else if constexpr (TR) {   // first pass of a frame: its posture rows become the instance's row of ptcur, which this pass's K2 reads
       if (a.ptcur) {
         const int PW = h.P * nq;
         for (int i = 0; i < nvalid; ++i) {
@@ -721,6 +793,48 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
   for (int s = 0; s < h.nsteps; ++s) {
     int n = prog[s * G + g];
     if (valid && n >= 0) fk_node<T>(P, n, qb, xs);
+    BIK_SYNCWARP();
+  }
+
+  // ---- held targets: a task held on this frame takes the held value in place of its sequence row; on the first pass of a
+  // run, the value is captured first, from q, into the held buffer (in the caller's precision), so that this pass's errors
+  // are taken against it.  A phase of its own after FK (the input loads and the frame loop keep their registers: fp32 spills
+  // otherwise); each lane handles the frames the frame loop gives it, and the CoM tasks the CoM phase's lane.
+  if constexpr (HO) {
+    if (valid) {
+      void* const held = static_cast<const K1HArgs&>(a).held;
+      const long long h0 = (long long)b * k1_tgt_words(h);
+      for (int f = g; f < h.F; f += G) {
+        const int s = k1h_hold(a, h, b, f);
+        if (s == 0) continue;
+        T* tg = ttile + (li * h.F + f) * 7;
+        if (s == 1) {
+          for (int k = 0; k < 7; ++k) tg[k] = ldin<T>(held, h0 + 7 * f + k, a.in64);
+          continue;
+        }
+        const FrameRec& fr = P.frame(f);
+        Q4<T> qf, qr, tq; V3<T> pf, pr, tp;
+        frame_pose<T>(fr.slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, &qf, &pf);
+        qr = qf; pr = pf;
+        if (fr.relative) frame_pose<T>(fr.rslot, KC<T>::frlpos(P, f), KC<T>::frlquat(P, f), xs, &qr, &pr);
+        held_frame_value<T>(fr.relative, qf, pf, qr, pr, &tq, &tp);
+        const T v[7] = {tq.w, tq.x, tq.y, tq.z, tp.x, tp.y, tp.z};
+        for (int k = 0; k < 7; ++k) { tg[k] = k1h_round<T>(v[k], a.in64); stout<T>(held, h0 + 7 * f + k, a.in64, tg[k]); }
+      }
+      if (g == 0)
+        for (int c = 0; c < h.C; ++c) {
+          const int s = k1h_hold(a, h, b, h.F + c);
+          if (s == 0) continue;
+          T* tg = ttile + IPW * h.F * 7 + (li * h.C + c) * 3;
+          if (s == 1) {
+            for (int k = 0; k < 3; ++k) tg[k] = ldin<T>(held, h0 + 7 * h.F + 3 * c + k, a.in64);
+            continue;
+          }
+          const V3<T> cv = model_com<T>(P, xs);
+          const T v[3] = {cv.x, cv.y, cv.z};
+          for (int k = 0; k < 3; ++k) { tg[k] = k1h_round<T>(v[k], a.in64); stout<T>(held, h0 + 7 * h.F + 3 * c + k, a.in64, tg[k]); }
+        }
+    }
     BIK_SYNCWARP();
   }
 

@@ -17,11 +17,12 @@ namespace bik {
 // points' per-instance task weights (K1Args::weights), or null.  posture_weights: the ..._weighted_ex entry points' per-instance
 // posture weights (K2PwArgs), or null.  bounds: the ..._bounded entry points' per-instance bounds (K2BdArgs), all three null
 // for none; held by value, so that the converge graph's key holds the three pointers.  coll: the ..._coll entry points'
-// per-instance collision pairs and distances (K1CArgs), all three null for none; held by value for the same reason.
+// per-instance collision pairs and distances (K1CArgs), all three null for none; held by value for the same reason.  hold: the
+// bik_track_hold entry points' [B][T][F + C + P] hold mask (K1HArgs), or null.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
   void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights; bik_bounds bounds;
-  bik_collision coll;
+  bik_collision coll; const uint8_t* hold;
 };
 inline bool has_bounds(const bik_bounds& bd) { return bd.lower || bd.upper || bd.vmax; }
 inline bool has_coll(const bik_collision& co) { return co.enabled || co.minimum_distance || co.detection_distance; }
@@ -30,18 +31,23 @@ inline bool has_coll(const bik_collision& co) { return co.enabled || co.minimum_
 // the caller's precision.  warm: [B][max(nu,1)] active-set guess.  done: [B] K2 leaves the instance alone.  cursor / step /
 // status: [B] frame each instance is on, steps taken in it (-1: no frames left) and its status (track only).
 // count = { steps taken (converge) or passes run (track), instances left, go }.  ptcur: [B][P][nq] posture targets of each
-// instance's current frame, in the caller's precision (track with a posture target sequence only, else unused).
+// instance's current frame, in the caller's precision (uses_ptcur only, else unused).  held: [B][7F + 3C] the held frame and
+// CoM targets, in the caller's precision (track with a hold mask only, else unused).
 struct ConvBufs {
   void *pk, *Gc, *hc, *dq;
   signed char* warm;
   int32_t *done, *cursor, *step, *status;
   int* count;
   void* ptcur;
+  void* held;
 };
 // bik_inputs.posture_batched names a posture target sequence (bik_track entry points only)
 inline bool posture_seq(const bik_inputs* in) {
   return in->posture_batched == BIK_POSTURE_SEQ_SHARED || in->posture_batched == BIK_POSTURE_SEQ_BATCHED;
 }
+// K1 keeps each instance's posture targets of its current frame in ptcur, which K2 reads: track mode with a posture target
+// sequence, or with a hold mask (a held posture target is the q its run started from)
+inline bool uses_ptcur(const ConvCall& c) { return c.track && (posture_seq(c.in) || c.hold); }
 // Per instance: elements of a pk / Gc / hc row (4 or 8 bytes each, by K1's precision) and bytes of warm.
 struct HandoffSizes { size_t pk, Gc, hc, warm; };
 inline HandoffSizes handoff_sizes(const PHeader& h) {
@@ -62,7 +68,7 @@ inline K1Args conv_k1_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   if (c.track) {
     a.cursor = s.cursor; a.tstep = s.step; a.lengths = c.lengths; a.T = c.T;
     a.q_traj = c.q_traj; a.traj_status = status; a.warm = s.warm;
-    if (posture_seq(in)) a.ptcur = s.ptcur;
+    if (uses_ptcur(c)) a.ptcur = s.ptcur;
   }
   return a;
 }
@@ -74,6 +80,14 @@ inline K1CArgs conv_k1c_args(const ConvCall& c, const ConvBufs& s, int32_t* stat
   a.enabled = c.coll.enabled; a.dmin = c.coll.minimum_distance; a.ddet = c.coll.detection_distance;
   return a;
 }
+// The same for the held-target instantiation of K1 (c.hold set, track mode); the collision arguments may be null.
+inline K1HArgs conv_k1h_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  K1HArgs a;
+  memset(&a, 0, sizeof a);
+  static_cast<K1CArgs&>(a) = conv_k1c_args(c, s, status);
+  a.hold = c.hold; a.held = s.held;
+  return a;
+}
 // K2 of a pass: solves and integrates the instances K1 left undone, and does nothing once the condition said stop.
 inline K2Args conv_k2_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
   const bik_inputs* in = c.in;
@@ -83,7 +97,7 @@ inline K2Args conv_k2_args(const ConvCall& c, const ConvBufs& s, int32_t* status
   a.Gc = s.Gc; a.hc = s.hc; a.gc64 = c.k1d; a.dt = c.dt; a.damping = c.damping; a.dq = s.dq; a.integrate = 1;
   a.status = c.track ? s.status : status;
   a.warm = s.warm; a.skip = s.done; a.gate = s.count + 2;
-  if (posture_seq(in)) { a.ptgt = s.ptcur; a.pbatched = 1; }   // K1 keeps each instance's current frame there
+  if (uses_ptcur(c)) { a.ptgt = s.ptcur; a.pbatched = 1; }   // K1 keeps each instance's current frame there
   return a;
 }
 // The same for the posture-weighted K2 (c.posture_weights set).  Track mode reads the row of each instance's current frame.

@@ -358,7 +358,8 @@ class Problem:
 
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-              check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None, bounds=None, collision=None):
+              check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None, bounds=None, collision=None,
+              hold=None):
         """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
         bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
@@ -371,7 +372,11 @@ class Problem:
         posture_weights: [B, T, P, nv] per-frame posture weights as in `converge` (bik_track_weighted_ex), or None.
         bounds: as in `converge`, [B, nv] each, one row per instance for every frame (bik_track_bounded), or None.
         collision: as in `converge` with one row per instance and frame, enabled [B, T, npairs] and the distances [B, T]
-        (bik_track_coll), or None."""
+        (bik_track_coll), or None.
+        hold: [B, T, H] bools, H = F + C + P: the frame-like tasks, then the CoM tasks, then the posture-type tasks, each in
+        the order of its targets (bik_track_hold), or None.  Over a run of frames where hold[b, :, k] is set, task k's target
+        is its value at the configuration instance b had when the run began (set_target_from_configuration), captured on the
+        device; its target rows on those frames are ignored."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         m = self.model
         B = q.shape[0]
@@ -393,6 +398,12 @@ class Problem:
         pw = self._posture_weights(posture_weights, q, B, T)
         bd, keep_bd = self._bounds(bounds, q, B)
         co, keep_co = self._collision(collision, q, B, T)
+        hd = None
+        if hold is not None:
+            H = self.F + self.Cn + self.P
+            hd = m._dev(hold, torch.uint8)
+            if hd.shape != (B, T, H):
+                raise ValueError(f"hold must be [B={B}, T={T}, H={H}] (frame, CoM and posture-type tasks), not {list(hd.shape)}")
         ln = None
         if lengths is not None:
             ln = m._dev(lengths, torch.int32).reshape(-1)
@@ -404,7 +415,11 @@ class Problem:
         passes = torch.zeros(1, device=q.device, dtype=torch.int32)
         args = (_ptr(ln), float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every),
                 q_traj.data_ptr(), iters.data_ptr(), status.data_ptr(), passes.data_ptr(), _stream())
-        if co is not None:
+        if hd is not None:
+            fn = self.lib.bik_track_hold64 if _is64(q) else self.lib.bik_track_hold
+            _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd),
+                          None if co is None else C.byref(co), hd.data_ptr(), *args))
+        elif co is not None:
             fn = self.lib.bik_track_coll64 if _is64(q) else self.lib.bik_track_coll
             _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
         elif bd is not None:

@@ -14,7 +14,7 @@ import numpy as np
 
 from ._abi import ProblemSpec
 from .configuration import Configuration
-from .exceptions import InvalidTarget, LimitDefinitionError
+from .exceptions import InvalidTarget, LimitDefinitionError, TargetNotSet
 from .limits import CollisionAvoidanceLimit, ConfigurationLimit, Limit, VelocityLimit
 from .tasks import ComTask, DampingTask, FrameTask, PostureTask, Task, problem_for
 
@@ -41,8 +41,8 @@ def _problem(configuration: Configuration, tasks: Sequence[Task], limits: Option
     return problem_for(configuration, ProblemSpec(tspecs, lspecs)), limits
 
 
-def _posture_targets(tasks: Sequence[Task], nq: int):
-    pt = [np.asarray(t._target()).reshape(-1, nq) for t in tasks if isinstance(t, PostureTask)]
+def _posture_targets(tasks: Sequence[Task], nq: int, target=lambda t: t._target()):
+    pt = [np.asarray(target(t)).reshape(-1, nq) for t in tasks if isinstance(t, PostureTask)]
     if not pt:
         return None
     nb = max(p.shape[0] for p in pt)
@@ -343,7 +343,7 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
              ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None, bounds=None,
-             collision=None):
+             collision=None, hold=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -376,6 +376,13 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     instance) or [B, T, npairs]; a distance is a float or [B] (every frame), [T] or [B, T] (a 2-D mask or a 1-D distance must
     then not leave B = T ambiguous).
 
+    `hold` maps a FrameTask, RelativeFrameTask, ComTask or PostureTask to a [T] or [B, T] mask of the frames it is held on.
+    Over each run of consecutive held frames the task's target is its value at the configuration the run begins from, as if
+    task.set_target_from_configuration(configuration) were called before the run's first frame: contact locking, a foot held
+    where it touched down for as long as the contact lasts.  The value is captured on the device; it replaces the task's
+    sequence or target on the held frames.  A task held on every frame of every instance needs neither a sequence nor a
+    target.  A DampingTask cannot be held.
+
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
     import torch
@@ -384,12 +391,37 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         if not isinstance(task, (FrameTask, ComTask, PostureTask)) or isinstance(task, DampingTask):
             raise InvalidTarget(f"track_ik takes target sequences for FrameTask, RelativeFrameTask, ComTask and PostureTask, "
                                 f"not {type(task).__name__}")
+    hold = hold or {}
+    for task in hold:
+        if not isinstance(task, (FrameTask, ComTask, PostureTask)) or isinstance(task, DampingTask) or task not in tasks:
+            raise InvalidTarget(f"track_ik holds FrameTask, RelativeFrameTask, ComTask and PostureTask targets of `tasks`, "
+                                f"not {type(task).__name__}")
     flat = configuration.flat
     q = configuration.q_device
     B, dev = q.shape[0], q.device
-    held = [t for t in tasks if isinstance(t, (FrameTask, ComTask)) and t not in targets]
-    for t in held:
-        t._target()   # TargetNotSet when a task has neither a sequence nor a target
+    masks = {}
+    for task, m in hold.items():
+        m = (m if isinstance(m, torch.Tensor) else torch.as_tensor(np.asarray(m))).to(device=dev) != 0
+        if m.ndim == 1:
+            m = m.unsqueeze(0).expand(B, -1)
+        if m.ndim != 2 or m.shape[0] != B or m.shape[1] < 1:
+            raise InvalidTarget(f"Expected a [T] or [{B}, T] hold mask for {type(task).__name__}, got {tuple(m.shape)}")
+        masks[task] = m
+    always = {t for t, m in masks.items() if bool(m.all())}   # held on every frame: its target rows are ignored
+
+    def target_of(t, fill):
+        try:
+            return np.asarray(t._target(), dtype=np.float64)
+        except TargetNotSet:
+            if t not in always:
+                raise
+            return np.asarray(fill, dtype=np.float64)
+
+    fills = {FrameTask: [1, 0, 0, 0, 0, 0, 0], ComTask: [0, 0, 0], PostureTask: np.asarray(flat.qpos0, dtype=np.float64)}
+    fill_of = lambda t: next(v for k, v in fills.items() if isinstance(t, k))
+    for t in tasks:
+        if isinstance(t, (FrameTask, ComTask)) and t not in targets:
+            target_of(t, fill_of(t))   # TargetNotSet when a task has neither a sequence nor a target (nor is always held)
     seqs, T = {}, None
     for task, seq in targets.items():
         k = 7 if isinstance(task, FrameTask) else (flat.nq if isinstance(task, PostureTask) else 3)
@@ -405,21 +437,25 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
             raise InvalidTarget(f"target sequences of different lengths: {T} and {s.shape[1]} frames")
         T = s.shape[1]
         seqs[task] = s
+    for task, m in masks.items():
+        if T is not None and m.shape[1] != T:
+            raise InvalidTarget(f"the hold mask of {type(task).__name__} has {m.shape[1]} frames, the sequences {T}")
+        T = m.shape[1]
     if T is None:
         raise InvalidTarget("track_ik needs at least one FrameTask / RelativeFrameTask / ComTask / PostureTask target sequence")
 
     def stacked(kind, k):
-        rows = [seqs[t] if t in seqs else torch.as_tensor(np.asarray(t._target(), dtype=np.float64).reshape(-1, 1, k), device=dev,
+        rows = [seqs[t] if t in seqs else torch.as_tensor(target_of(t, fill_of(t)).reshape(-1, 1, k), device=dev,
                                                           dtype=q.dtype).expand(B, T, k)
                 for t in tasks if isinstance(t, kind)]
         return torch.stack(rows, dim=2).contiguous() if rows else None
 
-    posture, posture_seq = _posture_targets(tasks, flat.nq), False
+    posture, posture_seq = _posture_targets(tasks, flat.nq, lambda t: target_of(t, fill_of(t))), False
     if any(isinstance(t, PostureTask) for t in seqs):
         # one [1 or B, T, nq] block per posture task (a sequence given without a batch dimension, or a held target shared by
         # the batch: 1); [T, P, nq] when every block is shared, else [B, T, P, nq]
         rows = [(seqs[t][:1] if seqs[t].stride(0) == 0 else seqs[t]) if t in seqs else
-                torch.as_tensor(np.asarray(t._target(), dtype=np.float64).reshape(-1, 1, flat.nq), device=dev, dtype=q.dtype).expand(-1, T, -1)
+                torch.as_tensor(target_of(t, fill_of(t)).reshape(-1, 1, flat.nq), device=dev, dtype=q.dtype).expand(-1, T, -1)
                 for t in tasks if isinstance(t, PostureTask)]
         lead = max(r.shape[0] for r in rows)
         posture = torch.stack([r.expand(lead, T, flat.nq) for r in rows], dim=2).contiguous()
@@ -436,10 +472,18 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
         if ln.shape != (B,):
             raise InvalidTarget(f"lengths must have shape ({B},), got {tuple(ln.shape)}")
+    hd = None
+    if masks:   # columns: frame-like tasks, CoM tasks, posture-type tasks, each in the order of `tasks`, as the targets are stacked
+        cols = [t for t in tasks if isinstance(t, FrameTask)] + [t for t in tasks if isinstance(t, ComTask)] + \
+               [t for t in tasks if isinstance(t, PostureTask)]
+        hd = torch.zeros((B, T, len(cols)), device=dev, dtype=torch.uint8)
+        for k, t in enumerate(cols):
+            if t in masks:
+                hd[:, :, k] = masks[t].to(torch.uint8)
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
                                           ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq,
-                                          posture_weights=pw, bounds=bd, collision=co)
+                                          posture_weights=pw, bounds=bd, collision=co, hold=hd)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran
