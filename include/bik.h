@@ -488,6 +488,47 @@ int bik_track_hold64(const bik_problem* problem, int B, int T, double* q, const 
                      const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
                      int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
 
+/* ---- per-instance frame placement --------------------------------------------------------------------------------------
+ * bik_step_coll / bik_converge_coll with one more argument, `placement`, right after `coll`, and bik_track_hold with it right
+ * after `hold`: each instance puts each frame task's frame at its own pose on the task's tree node, as a mink user who moves
+ * model.site_pos / site_quat (geom_pos / geom_quat) between solves does.  Marker retargeting (one marker placement per
+ * performer), tool or TCP offsets, and fingertip contact points are the typical uses.
+ *   placement  device, [B][F][7] in the inputs' precision (bik_inputs.f64), F = number of FRAME + RELATIVE_FRAME tasks in the
+ *              order of frame_targets.  Row b*F + f is wxyz xyz, laid out as frame_targets: the pose of task f's frame in its
+ *              tree node, what bik_task_desc.frame.quat / pos would be.  bik_track_placed uses row b*F + f on every frame.
+ *              A NULL `placement` runs exactly what bik_step_coll / bik_converge_coll / bik_track_hold run, through the same
+ *              kernels, bit for bit.  Non-NULL on a problem without frame-like tasks is BIK_ERR_INVALID.
+ *   `weights`, `posture_weights`, `bounds`, `coll`, `hold` and `lengths` as in those entry points.
+ *   Instance b runs what a problem built with frame poses row b runs.  The node stays the problem's (a placement moves a frame
+ *   on its body, never onto another body), and a RELATIVE_FRAME task's root keeps the problem's placement.  A row that holds
+ *   exactly what the problem image would hold for that pose (the builder divides the quaternion by its norm in double, then
+ *   stores both in K1's precision) gives that problem's dq, q, iters, status and passes bit for bit; a quaternion that is not
+ *   of unit length is used as given, not renormalised.  The convergence test takes the placed frames' errors; a held FRAME
+ *   task captures the world pose of its placed frame, a held RELATIVE_FRAME task that frame's pose in its root.
+ *   A row with a non-finite element keeps the problem's placement for that task and instance and sets BIK_STATUS_NONFINITE on
+ *   the instance (bik_track_placed: on every frame the instance runs).
+ *   bik_fk_jac, bik_solve, bik_limits_box and bik_step_host have no placed form. */
+int bik_step_placed(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                    const bik_bounds* bounds, const bik_collision* coll, const void* placement, float dt, double damping, int nsteps,
+                    int integrate, float* dq, int32_t* status, void* stream);
+int bik_step_placed64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                      const bik_bounds* bounds, const bik_collision* coll, const void* placement, double dt, double damping, int nsteps,
+                      int integrate, double* dq, int32_t* status, void* stream);
+int bik_converge_placed(const bik_problem* problem, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                        const bik_bounds* bounds, const bik_collision* coll, const void* placement, float dt, double damping, int max_iters,
+                        float pos_threshold, float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_converge_placed64(const bik_problem* problem, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                          const bik_bounds* bounds, const bik_collision* coll, const void* placement, double dt, double damping, int max_iters,
+                          double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream);
+int bik_track_placed(const bik_problem* problem, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                     const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold, const void* placement, const int32_t* lengths,
+                     float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj,
+                     int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+int bik_track_placed64(const bik_problem* problem, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                       const void* posture_weights, const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold,
+                       const void* placement, const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
+                       double ori_threshold, int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream);
+
 /* Measurement aid for the K2 roofline (bench.py): sustained fused-multiply-add throughput of the CUDA cores of `device`
  * in TFLOP/s (fp32 or fp64; 16 independent chains per thread, every SM filled), best of `repeats` event-timed launches. */
 int bik_measure_fma_peak(int device, int use_double, int repeats, double* tflops);

@@ -21,7 +21,8 @@ EXPORTS = ["bik_version", "bik_last_error", "bik_model_create", "bik_model_destr
            "bik_step_weighted_ex64", "bik_converge_weighted_ex64", "bik_track_weighted_ex64", "bik_step_bounded",
            "bik_converge_bounded", "bik_track_bounded", "bik_step_bounded64", "bik_converge_bounded64", "bik_track_bounded64",
            "bik_step_coll", "bik_converge_coll", "bik_track_coll", "bik_step_coll64", "bik_converge_coll64", "bik_track_coll64",
-           "bik_track_hold", "bik_track_hold64"]
+           "bik_track_hold", "bik_track_hold64", "bik_step_placed", "bik_converge_placed", "bik_track_placed",
+           "bik_step_placed64", "bik_converge_placed64", "bik_track_placed64"]
 
 
 class BikError(RuntimeError):
@@ -101,6 +102,11 @@ def load():
         args = getattr(lib, name).argtypes
         at = args.index(C.POINTER(BikCollision)) + 1
         getattr(lib, name.replace("_coll", "_hold")).argtypes = args[:at] + [vp] + args[at:]
+    # per-instance frame placement: the placement rows after the collision arguments (bik_track: after the hold mask)
+    for name in ("bik_step_coll", "bik_converge_coll", "bik_step_coll64", "bik_converge_coll64", "bik_track_hold", "bik_track_hold64"):
+        args = getattr(lib, name).argtypes
+        at = args.index(C.POINTER(BikCollision)) + (2 if "_hold" in name else 1)
+        getattr(lib, name.replace("_coll", "_placed").replace("_hold", "_placed")).argtypes = args[:at] + [vp] + args[at:]
     _lib = lib
     return lib
 

@@ -314,12 +314,13 @@ extern "C" int bik_frame_jacobian64(const bik_model* model, int B, const double*
 
 // track: a bik_track entry point, the only ones that take a posture target sequence
 // bounds: the ..._bounded entry points' bounds (as from bounds_of), or null; coll: the ..._coll entry points' collision
-// arguments (as from coll_of), or null
+// arguments (as from coll_of), or null; placement: the ..._placed entry points' frame placements, or null
 static int check_inputs(const bik_problem* p, const bik_inputs* in, bool need_q, int f64, bool track = false, const void* posture_weights = nullptr,
-                        const bik_bounds* bounds = nullptr, const bik_collision* coll = nullptr) {
+                        const bik_bounds* bounds = nullptr, const bik_collision* coll = nullptr, const void* placement = nullptr) {
   if (!p || !in) return bik_fail(BIK_ERR_INVALID, "null argument");
   const PHeader& h = p->h;
   if (coll && h.npairs == 0) return bik_fail(BIK_ERR_INVALID, "coll given for a problem without a CollisionAvoidanceLimit");
+  if (placement && h.F == 0) return bik_fail(BIK_ERR_INVALID, "placement given for a problem without a FrameTask or RelativeFrameTask");
   if (posture_weights && h.P == 0) return bik_fail(BIK_ERR_INVALID, "posture_weights given for a problem without a PostureTask or DampingTask");
   if (bounds && (bounds->lower || bounds->upper) && h.ncfg == 0)
     return bik_fail(BIK_ERR_INVALID, "bounds.lower / bounds.upper given for a problem without a ConfigurationLimit");
@@ -480,9 +481,10 @@ int HostStaging::reserve(const PHeader& h, size_t B, size_t pt_elems) {
 // One or more solve_ik steps on device buffers: per step K1 (check_limits + FK + packed task rows + collision rows) and
 // K2 (QP + integrate).  Caller holds p->mu and has reserved the hand-off for `k1d ? 8 : 4`-byte elements.
 // bounds: per-instance bounds (the bounded K2), or null.  coll: per-instance collision pairs and distances (k1c_kernel), or null.
+// placement: per-instance frame placements (k1p_kernel, with coll's members or null ones), or null.
 static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
-                     const bik_bounds* bounds, const bik_collision* coll, double dt, double damping, int nsteps, int integrate, void* dq, int32_t* status, int io64, bool k1d,
-                     cudaStream_t st) {
+                     const bik_bounds* bounds, const bik_collision* coll, const void* placement, double dt, double damping, int nsteps, int integrate, void* dq,
+                     int32_t* status, int io64, bool k1d, cudaStream_t st) {
   // hand-off rows [ws_off, ws_off + B): chunks of one batch may be in flight on different streams (bik_step_host)
   const HandoffSizes n = handoff_sizes(p->h);
   const size_t es = k1d ? 8 : 4;
@@ -500,7 +502,14 @@ static int step_core(bik_problem* p, int B, size_t ws_off, void* q, const bik_in
     a1.dt = dt; a1.pk = pk; a1.Gc = Gc; a1.hc = hc; a1.weights = weights;
     a1.status = status; a1.accumulate = s > 0; a1.tol = 1e-6f;   // Configuration.check_limits(safety_break=False) of solve_ik.py:99
     int rc = BIK_OK;
-    if (phase != 2 && coll) {
+    if (phase != 2 && placement) {
+      K1PArgs pa;
+      memset(&pa, 0, sizeof pa);
+      static_cast<K1Args&>(pa) = a1;
+      if (coll) { pa.enabled = coll->enabled; pa.dmin = coll->minimum_distance; pa.ddet = coll->detection_distance; }
+      pa.placement = placement;
+      rc = bik_launch_k1(p, pa, k1d, st);
+    } else if (phase != 2 && coll) {
       K1CArgs ca;
       memset(&ca, 0, sizeof ca);
       static_cast<K1Args&>(ca) = a1;
@@ -543,13 +552,14 @@ static const bik_bounds* bounds_of(const bik_bounds* bounds) { return bounds && 
 // call runs what the ..._bounded call runs.
 static const bik_collision* coll_of(const bik_collision* coll) { return coll && has_coll(*coll) ? coll : nullptr; }
 
+// placement: the ..._placed entry points' frame placements, or null (what the ..._coll entry points run).
 static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                        const bik_bounds* bounds, const bik_collision* coll, double dt, double damping, int nsteps, int integrate, void* dq, int32_t* status, int f64,
-                       void* stream) {
+                       void* stream, const void* placement = nullptr) {
   if (B == 0 && cp) return BIK_OK;
   bounds = bounds_of(bounds);
   coll = coll_of(coll);
-  int rc = check_inputs(cp, in, false, f64, false, posture_weights, bounds, coll);
+  int rc = check_inputs(cp, in, false, f64, false, posture_weights, bounds, coll, placement);
   if (rc) return rc;
   if (!q || !dq || B < 0 || nsteps < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   bik_problem* p = const_cast<bik_problem*>(cp);
@@ -562,7 +572,7 @@ static int step_common(const bik_problem* cp, int B, void* q, const bik_inputs* 
   rc = ws_acquire(p, st);
   if (rc) return rc;
   // (status needs no clearing: K1's fused check_limits assigns it on the first step, everything later ORs into it)
-  return ws_release(p, st, step_core(p, B, 0, q, in, weights, posture_weights, bounds, coll, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
+  return ws_release(p, st, step_core(p, B, 0, q, in, weights, posture_weights, bounds, coll, placement, dt, damping, nsteps, integrate, dq, status, f64, k1d, st));
 }
 extern "C" int bik_step(const bik_problem* p, int B, float* q, const bik_inputs* in, float dt, double damping, int nsteps, int integrate, float* dq,
                         int32_t* status, void* stream) {
@@ -608,6 +618,16 @@ extern "C" int bik_step_coll64(const bik_problem* p, int B, double* q, const bik
                                int32_t* status, void* stream) {
   return step_common(p, B, q, in, weights, posture_weights, bounds, coll, dt, damping, nsteps, integrate, dq, status, 1, stream);
 }
+extern "C" int bik_step_placed(const bik_problem* p, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                               const bik_bounds* bounds, const bik_collision* coll, const void* placement, float dt, double damping, int nsteps,
+                               int integrate, float* dq, int32_t* status, void* stream) {
+  return step_common(p, B, q, in, weights, posture_weights, bounds, coll, dt, damping, nsteps, integrate, dq, status, 0, stream, placement);
+}
+extern "C" int bik_step_placed64(const bik_problem* p, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                 const bik_bounds* bounds, const bik_collision* coll, const void* placement, double dt, double damping, int nsteps,
+                                 int integrate, double* dq, int32_t* status, void* stream) {
+  return step_common(p, B, q, in, weights, posture_weights, bounds, coll, dt, damping, nsteps, integrate, dq, status, 1, stream, placement);
+}
 
 extern "C" int bik_problem_describe(const bik_problem* p, double damping, char* buf, size_t cap) {
   if (!p) return bik_fail(BIK_ERR_INVALID, "null argument");
@@ -643,8 +663,9 @@ static ConvBufs conv_bufs(const bik_problem* p) {
 static int converge_pass(bik_problem* p, const ConvCall& c, int32_t* status, cudaGraphConditionalHandle handle, int use_handle, cudaStream_t st) {
   const ConvBufs s = conv_bufs(p);
   conv_tick_kernel<<<1, 1, 0, st>>>(c.track, s.count);
-  int rc = c.hold ? bik_launch_k1(p, conv_k1h_args(c, s, status), c.k1d, st)
-                  : (has_coll(c.coll) ? bik_launch_k1(p, conv_k1c_args(c, s, status), c.k1d, st) : bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st));
+  int rc = c.placement ? bik_launch_k1(p, conv_k1p_args(c, s, status), c.k1d, st)
+           : c.hold ? bik_launch_k1(p, conv_k1h_args(c, s, status), c.k1d, st)
+           : (has_coll(c.coll) ? bik_launch_k1(p, conv_k1c_args(c, s, status), c.k1d, st) : bik_launch_k1(p, conv_k1_args(c, s, status), c.k1d, st));
   if (rc) return rc;
   conv_cond_kernel<<<1, 1, 0, st>>>(c.track, c.max_iters, s.count, handle, use_handle);
   if (has_bounds(c.bounds)) rc = dispatch_k2(p, conv_k2_bd_args(c, s, status), st);
@@ -747,13 +768,14 @@ static int converge_run(bik_problem* p, const ConvCall& c, int check_every, int3
   return ws_release(p, st, BIK_OK);
 }
 
+// placement: the ..._placed entry points' frame placements, or null.
 static int converge_common(const bik_problem* cp, int B, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                            const bik_bounds* bounds, const bik_collision* coll, double dt, double damping, int max_iters, double pos_threshold, double ori_threshold,
-                           int check_every, int32_t* iters, int32_t* status, int io64, void* stream) {
+                           int check_every, int32_t* iters, int32_t* status, int io64, void* stream, const void* placement = nullptr) {
   if (B == 0 && cp) return BIK_OK;
   bounds = bounds_of(bounds);
   coll = coll_of(coll);
-  int rc = check_inputs(cp, in, false, io64, false, posture_weights, bounds, coll);
+  int rc = check_inputs(cp, in, false, io64, false, posture_weights, bounds, coll, placement);
   if (rc) return rc;
   if (!q || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (check_every < 1) check_every = 1;
@@ -765,6 +787,7 @@ static int converge_common(const bik_problem* cp, int B, void* q, const bik_inpu
   c.weights = weights; c.posture_weights = posture_weights;
   if (bounds) c.bounds = *bounds;
   if (coll) c.coll = *coll;
+  c.placement = placement;
   return converge_run(p, c, check_every, nullptr, static_cast<cudaStream_t>(stream));
 }
 extern "C" int bik_converge(const bik_problem* cp, int B, float* q, const bik_inputs* in, float dt, double damping, int max_iters, float pos_threshold,
@@ -821,19 +844,32 @@ extern "C" int bik_converge_coll64(const bik_problem* cp, int B, double* q, cons
   return converge_common(cp, B, q, in, weights, posture_weights, bounds, coll, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1,
                          stream);
 }
+extern "C" int bik_converge_placed(const bik_problem* cp, int B, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                   const bik_bounds* bounds, const bik_collision* coll, const void* placement, float dt, double damping, int max_iters,
+                                   float pos_threshold, float ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, weights, posture_weights, bounds, coll, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 0,
+                         stream, placement);
+}
+extern "C" int bik_converge_placed64(const bik_problem* cp, int B, double* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                     const bik_bounds* bounds, const bik_collision* coll, const void* placement, double dt, double damping, int max_iters,
+                                     double pos_threshold, double ori_threshold, int check_every, int32_t* iters, int32_t* status, void* stream) {
+  return converge_common(cp, B, q, in, weights, posture_weights, bounds, coll, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, iters, status, 1,
+                         stream, placement);
+}
 
 // The examples' outer loop: for each frame of a target sequence, the bik_converge loop, every instance on its own cursor.
 // One pass works like a bik_converge pass; K1's test, when it ends an instance's frame, records that frame's results and
 // moves the instance to its next frame (K1Args, track mode).  The loop ends when no instance has frames left.
-// hold: the bik_track_hold entry points' hold mask, or null.
+// hold: the bik_track_hold entry points' hold mask, or null.  placement: the bik_track_placed entry points' frame placements, or
+// null.
 static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_inputs* in, const void* weights, const void* posture_weights,
                         const bik_bounds* bounds, const bik_collision* coll, const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
                         double ori_threshold, int check_every, void* q_traj, int32_t* iters, int32_t* status, int32_t* passes, int io64, void* stream,
-                        const uint8_t* hold = nullptr) {
+                        const uint8_t* hold = nullptr, const void* placement = nullptr) {
   if (B == 0 && cp) return BIK_OK;
   bounds = bounds_of(bounds);
   coll = coll_of(coll);
-  int rc = check_inputs(cp, in, false, io64, true, posture_weights, bounds, coll);
+  int rc = check_inputs(cp, in, false, io64, true, posture_weights, bounds, coll, placement);
   if (rc) return rc;
   if (!q || !q_traj || !iters || B < 0 || max_iters < 1) return bik_fail(BIK_ERR_INVALID, "bad argument");
   if (T < 1) return bik_fail(BIK_ERR_INVALID, "T must be at least 1");
@@ -856,6 +892,7 @@ static int track_common(const bik_problem* cp, int B, int T, void* q, const bik_
   if (bounds) c.bounds = *bounds;
   if (coll) c.coll = *coll;
   c.hold = hold;
+  c.placement = placement;
   return converge_run(p, c, check_every, passes, st);
 }
 extern "C" int bik_track(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const int32_t* lengths, float dt, double damping,
@@ -930,6 +967,20 @@ extern "C" int bik_track_hold64(const bik_problem* cp, int B, int T, double* q, 
                                 int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
   return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
                       iters, status, passes, 1, stream, hold);
+}
+extern "C" int bik_track_placed(const bik_problem* cp, int B, int T, float* q, const bik_inputs* in, const void* weights, const void* posture_weights,
+                                const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold, const void* placement, const int32_t* lengths,
+                                float dt, double damping, int max_iters, float pos_threshold, float ori_threshold, int check_every, float* q_traj,
+                                int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 0, stream, hold, placement);
+}
+extern "C" int bik_track_placed64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const void* weights,
+                                  const void* posture_weights, const bik_bounds* bounds, const bik_collision* coll, const uint8_t* hold,
+                                  const void* placement, const int32_t* lengths, double dt, double damping, int max_iters, double pos_threshold,
+                                  double ori_threshold, int check_every, double* q_traj, int32_t* iters, int32_t* status, int32_t* passes, void* stream) {
+  return track_common(cp, B, T, q, in, weights, posture_weights, bounds, coll, lengths, dt, damping, max_iters, pos_threshold, ori_threshold, check_every, q_traj,
+                      iters, status, passes, 1, stream, hold, placement);
 }
 extern "C" int bik_track64(const bik_problem* cp, int B, int T, double* q, const bik_inputs* in, const int32_t* lengths, double dt, double damping,
                            int max_iters, double pos_threshold, double ori_threshold, int check_every, double* q_traj, int32_t* iters,
@@ -1024,7 +1075,7 @@ extern "C" int bik_step_host(const bik_problem* cp, int B, float* q_host, const 
     bik_inputs din = *in;
     din.q = hq + o * nq; din.frame_targets = hft + o * h.F * 7; din.com_targets = hct + o * h.C * 3;
     din.posture_targets = in->posture_batched ? hpt + o * (size_t)h.P * nq : hpt;
-    rc = step_core(p, (int)n, o, hq + o * nq, &din, nullptr, nullptr, nullptr, nullptr, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
+    rc = step_core(p, (int)n, o, hq + o * nq, &din, nullptr, nullptr, nullptr, nullptr, nullptr, dt, damping, nsteps, integrate, hdq + o * nv, status_host ? hst + o : nullptr, 0, k1d, s_cmp);
     if (rc) return rc;
     CUDA_OK(cudaEventRecord(hb.hev[2 * ci + 1], s_cmp));
     mark(s_cmp);

@@ -182,6 +182,7 @@ int bik_launch_geometry(const void* kern, const bik_model* m, size_t smem, int t
 int bik_launch_k1(const bik_problem* p, const bik::K1Args& a, bool use_double, cudaStream_t st);
 int bik_launch_k1(const bik_problem* p, const bik::K1CArgs& a, bool use_double, cudaStream_t st);   // per-instance collision pairs (k1c_kernel)
 int bik_launch_k1(const bik_problem* p, const bik::K1HArgs& a, bool use_double, cudaStream_t st);   // held targets (k1h_kernel)
+int bik_launch_k1(const bik_problem* p, const bik::K1PArgs& a, bool use_double, cudaStream_t st);   // frame placement (k1p_kernel)
 int bik_launch_fk(const bik_model* m, const bik::FkArgs& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2Args& a, cudaStream_t st);
 int bik_launch_k2_general(const bik_problem* p, const bik::K2PwArgs& a, cudaStream_t st);   // posture-weighted instantiations

@@ -121,6 +121,45 @@ __global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1
   }
 }
 
+// Per-instance frame placement (K1PArgs): the ..._placed entry points, step and converge (TR = false) or track (TR), with held
+// targets in track (HO); the collision arguments may be null.  A kernel of its own for the same reason.
+template <typename T, int G, bool TR, bool HO>
+__global__ void __launch_bounds__(128, sizeof(T) == 4 ? BIK_K1_MINBLOCKS : 2) k1p_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, K1PArgs a) {
+  static_assert(!HO || TR, "held targets are a track-mode feature");
+  constexpr bool PK = true;
+  extern __shared__ __align__(16) uint32_t smem[];
+  __shared__ __align__(8) uint64_t bar;
+  __shared__ __align__(8) uint64_t pbar[4];   // one input-pipeline barrier per warp
+  stage_image(smem, gimage, words, &bar, use_tma);
+  PView P{smem};
+  const PHeader& h = P.h();
+  constexpr int IPW = 32 / G;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  T* wsm = reinterpret_cast<T*>(smem + words) + (size_t)warp * k1_warp_words(h, IPW);
+  const int ntiles = (a.B + IPW - 1) / IPW, stride = gridDim.x * nwarps;
+  int tile = blockIdx.x * nwarps + warp;
+  // Input pipeline: tile t computes its Jacobian columns while the q rows and targets of tile t + stride arrive by bulk async
+  // copy (BIK_USE_TMA=0 turns it off together with the staged image: plain loads at the top of every tile).
+  K1Pipe pipe{&pbar[warp], 0u, -1};
+  K1Pipe* pp = use_tma ? &pipe : nullptr;
+  if (pp) {
+    if (lane == 0) {
+      mbar_init(pipe.bar, 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    if (tile < ntiles && k1_tile_bulk_ok<T, TR>(h, a, tile * IPW, IPW)) {
+      T* qtile = wsm + k1_qtile_offset(h, IPW);
+      if (lane == 0) k1_pipe_arm<T, TR>(h, a, tile * IPW, IPW, &pipe, qtile, qtile + ((IPW * h.nq + 3) & ~3));
+      pipe.armed = tile * IPW;
+    }
+  }
+  for (; tile < ntiles; tile += stride) {
+    const int next = tile + stride < ntiles ? (tile + stride) * IPW : -1;
+    k1_warp_tile<T, G, 32, PK, TR, true, HO, true>(P, a, tile * IPW, wsm, lane, pp, next);
+  }
+}
+
 template <typename T, int G>
 __global__ void __launch_bounds__(128) fk_kernel(const uint32_t* __restrict__ gimage, int words, int use_tma, FkArgs a) {
   extern __shared__ __align__(16) uint32_t smem[];
@@ -134,7 +173,7 @@ __global__ void __launch_bounds__(128) fk_kernel(const uint32_t* __restrict__ gi
   for (int tile = blockIdx.x * nwarps + warp; tile < ntiles; tile += gridDim.x * nwarps) fk_warp_tile<T, G, 32>(P, a, tile * IPW, wsm, lane);
 }
 
-// Launch K1 kernel `kern` (a k1_kernel, k1c_kernel or k1h_kernel instantiation of scalar type T and G lanes per instance).
+// Launch K1 kernel `kern` (a k1_kernel, k1c_kernel, k1h_kernel or k1p_kernel instantiation of scalar type T and G lanes per instance).
 template <typename T, int G, typename A>
 static int launch_k1_kernel(const bik_problem* p, void (*kern)(const uint32_t*, int, int, A), const A& a, cudaStream_t st) {
   const PHeader& h = p->h;
@@ -166,6 +205,11 @@ static int launch_k1(const bik_problem* p, const K1HArgs& a, cudaStream_t st) {
   const bool co = a.enabled || a.dmin || a.ddet;
   return launch_k1_kernel<T, G>(p, co ? k1h_kernel<T, G, true> : k1h_kernel<T, G, false>, a, st);
 }
+template <typename T, int G>
+static int launch_k1(const bik_problem* p, const K1PArgs& a, cudaStream_t st) {
+  if (!a.cursor) return launch_k1_kernel<T, G>(p, k1p_kernel<T, G, false, false>, a, st);
+  return launch_k1_kernel<T, G>(p, a.hold ? k1p_kernel<T, G, true, true> : k1p_kernel<T, G, true, false>, a, st);
+}
 template <typename T, typename A>
 static int dispatch_k1(const bik_problem* p, const A& a, cudaStream_t st) {
   switch (p->h.G) {
@@ -189,6 +233,12 @@ int bik_launch_k1(const bik_problem* p, const K1CArgs& a, bool use_double, cudaS
 int bik_launch_k1(const bik_problem* p, const K1HArgs& a, bool use_double, cudaStream_t st) {
   if (!use_double && a.in64) return bik_fail(BIK_ERR_INVALID, "fp64 inputs need the fp64 instantiation of K1");
   if (!a.pk || !a.cursor || !a.held) return bik_fail(BIK_ERR_INVALID, "held targets need track mode's packed hand-off and a held buffer");
+  return use_double ? dispatch_k1<double>(p, a, st) : dispatch_k1<float>(p, a, st);
+}
+int bik_launch_k1(const bik_problem* p, const K1PArgs& a, bool use_double, cudaStream_t st) {
+  if (!use_double && a.in64) return bik_fail(BIK_ERR_INVALID, "fp64 inputs need the fp64 instantiation of K1");
+  if (!a.pk || !a.placement) return bik_fail(BIK_ERR_INVALID, "frame placement needs the packed hand-off and a placement buffer");
+  if (a.hold && (!a.cursor || !a.held)) return bik_fail(BIK_ERR_INVALID, "held targets need track mode and a held buffer");
   return use_double ? dispatch_k1<double>(p, a, st) : dispatch_k1<float>(p, a, st);
 }
 

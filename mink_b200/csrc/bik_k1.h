@@ -206,6 +206,15 @@ BIK_HD int k1h_hold(const K1Args& a, const PHeader& h, int b, int k) {
   if (!hold[row * H + k]) return 0;
   return a.tstep[b] == 0 && (a.cursor[b] == 0 || !hold[(row - 1) * H + k]) ? 2 : 1;
 }
+// The arguments of the placement instantiation (k1p_kernel, k1_warp_tile<..., CO = true, HO, PL = true>): the ..._placed entry
+// points; the collision and hold members as in K1CArgs / K1HArgs, each may be null (HO: hold and held set).  placement [B][F][7],
+// in the inputs' element type: row b*F + f is the pose (wxyz, xyz) of frame task f's frame in its tree node for instance b, in
+// place of the problem's (KC<T>::flpos / flquat), on every frame in track mode.  It is used as given (a quaternion is not
+// renormalised); a row with a non-finite element falls back to the problem's and sets BIK_STATUS_NONFINITE on the instance.
+// A RELATIVE_FRAME task's root keeps the problem's placement.
+struct K1PArgs : K1HArgs {
+  const void* placement;
+};
 // v as the caller's precision holds it (a captured target is stored there, as a target the caller passed would be)
 template <typename T> BIK_HD T k1h_round(T v, int is64) { return sizeof(T) == 8 && !is64 ? T(float(v)) : v; }
 // row of instance b in the K1CArgs buffers: b, or in track mode that of its current frame
@@ -369,6 +378,18 @@ BIK_HD void frame_pose(int node, V3<T> lpos, Q4<T> lquat, const T* xs, Q4<T>* qf
   Q4<T> nq = ld_q(xs + 7 * node);
   *qf = qnormalize(qmul(nq, lquat));
   *pf = ld_v(xs + 7 * node + 4) + qrot(nq, lpos);
+}
+// frame_pose of frame task f's frame (tree state row `slot`) for instance b of a K1PArgs call: at the instance's placement row
+// where all seven values are finite, else at the problem's
+template <typename T>
+BIK_HD void k1p_frame_pose(const PView& P, const K1Args& a, int b, int f, int slot, const T* xs, Q4<T>* qf, V3<T>* pf) {
+  const long long r = ((long long)b * P.h().F + f) * 7;
+  const void* pl = static_cast<const K1PArgs&>(a).placement;
+  T v[7];
+  bool fin = true;
+  for (int k = 0; k < 7; ++k) { v[k] = ldin<T>(pl, r + k, a.in64); fin = fin && v[k] - v[k] == T(0); }
+  if (fin) frame_pose<T>(slot, v3<T>(v[4], v[5], v[6]), q4<T>(v[0], v[1], v[2], v[3]), xs, qf, pf);
+  else frame_pose<T>(slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, qf, pf);
 }
 // root^-1 * frame for two world poses as bik_fk reports them, composed as mink's SE3 does (root.inverse() @ frame): the pose a
 // held RELATIVE_FRAME task captures (RelativeFrameTask.set_target_from_configuration)
@@ -640,11 +661,13 @@ template <> BIK_HD void store6<double>(double* o, V3<double> top, V3<double> bot
 // TR (compile time, with PK): track mode of bik_track (see K1Args); a third instantiation, so the other two are unchanged.
 // CO (compile time, with PK): `a` is a K1CArgs, per-instance collision pairs and distances (the ..._coll entry points).
 // HO (compile time, with TR): `a` is a K1HArgs, held targets (the bik_track_hold entry points).
-template <typename T, int G, int W, bool PK, bool TR = false, bool CO = false, bool HO = false>
+// PL (compile time, with CO): `a` is a K1PArgs, per-instance frame placement (the ..._placed entry points).
+template <typename T, int G, int W, bool PK, bool TR = false, bool CO = false, bool HO = false, bool PL = false>
 BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int lane, K1Pipe* pipe = nullptr, int next_inst0 = -1) {
   static_assert(!TR || PK, "track mode writes the packed hand-off");
   static_assert(!CO || PK, "per-instance collision pairs write the packed hand-off");
   static_assert(!HO || TR, "held targets are a track-mode feature");
+  static_assert(!PL || CO, "frame placement runs with the collision arguments");
   const PHeader& h = P.h();
   constexpr int IPW = W / G;
   const int nv = h.nv, nq = h.nq, K = h.K;
@@ -771,6 +794,14 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
           if (!k1c_finite<T>(ca.dmin, r, a.in64) || !k1c_finite<T>(ca.ddet, r, a.in64)) bad |= 4;
         }
       }
+      if constexpr (PL) {   // a non-finite placement: BIK_STATUS_NONFINITE (the problem's placement is used)
+        const void* pl = static_cast<const K1PArgs&>(a).placement;
+        const long long r0 = (long long)(inst0 + i) * h.F * 7;
+        for (int k = lane; k < h.F * 7; k += W) {
+          const T v = ldin<T>(pl, r0 + k, a.in64);
+          if (!(v - v == T(0))) bad |= 4;
+        }
+      }
       if (bad) {
 #if defined(__CUDA_ARCH__)
         atomicOr(&sflag[i], bad);
@@ -814,7 +845,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
         }
         const FrameRec& fr = P.frame(f);
         Q4<T> qf, qr, tq; V3<T> pf, pr, tp;
-        frame_pose<T>(fr.slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, &qf, &pf);
+        if constexpr (PL) k1p_frame_pose<T>(P, a, b, f, fr.slot, xs, &qf, &pf);
+        else frame_pose<T>(fr.slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, &qf, &pf);
         qr = qf; pr = pf;
         if (fr.relative) frame_pose<T>(fr.rslot, KC<T>::frlpos(P, f), KC<T>::frlquat(P, f), xs, &qr, &pr);
         held_frame_value<T>(fr.relative, qf, pf, qr, pr, &tq, &tp);
@@ -845,7 +877,8 @@ BIK_HD void k1_warp_tile(const PView& P, const K1Args& a, int inst0, T* wsm, int
     for (int f = g; f < h.F; f += G) {
       const FrameRec& fr = P.frame(f);
       Q4<T> qf; V3<T> pf, ev, ew; M3<T> A1, A2;
-      frame_pose<T>(fr.slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, &qf, &pf);
+      if constexpr (PL) k1p_frame_pose<T>(P, a, b, f, fr.slot, xs, &qf, &pf);
+      else frame_pose<T>(fr.slot, KC<T>::flpos(P, f), KC<T>::flquat(P, f), xs, &qf, &pf);
       T* sc = fsc + (li * h.F + f) * FS;
       const T* tg = ttile + (li * h.F + f) * 7;
       Q4<T> tq = q4<T>(tg[0], tg[1], tg[2], tg[3]);

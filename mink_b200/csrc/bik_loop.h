@@ -18,11 +18,12 @@ namespace bik {
 // posture weights (K2PwArgs), or null.  bounds: the ..._bounded entry points' per-instance bounds (K2BdArgs), all three null
 // for none; held by value, so that the converge graph's key holds the three pointers.  coll: the ..._coll entry points'
 // per-instance collision pairs and distances (K1CArgs), all three null for none; held by value for the same reason.  hold: the
-// bik_track_hold entry points' [B][T][F + C + P] hold mask (K1HArgs), or null.
+// bik_track_hold entry points' [B][T][F + C + P] hold mask (K1HArgs), or null.  placement: the ..._placed entry points' [B][F][7]
+// frame placements (K1PArgs), or null.
 struct ConvCall {
   int B, T, max_iters; double dt, pos, ori; double damping; void* q; const bik_inputs* in; const int32_t* lengths;
   void* q_traj; int32_t *iters, *status; bool track, k1d, io64; const void* weights; const void* posture_weights; bik_bounds bounds;
-  bik_collision coll; const uint8_t* hold;
+  bik_collision coll; const uint8_t* hold; const void* placement;
 };
 inline bool has_bounds(const bik_bounds& bd) { return bd.lower || bd.upper || bd.vmax; }
 inline bool has_coll(const bik_collision& co) { return co.enabled || co.minimum_distance || co.detection_distance; }
@@ -86,6 +87,16 @@ inline K1HArgs conv_k1h_args(const ConvCall& c, const ConvBufs& s, int32_t* stat
   memset(&a, 0, sizeof a);
   static_cast<K1CArgs&>(a) = conv_k1c_args(c, s, status);
   a.hold = c.hold; a.held = s.held;
+  return a;
+}
+// The same for the placement instantiation of K1 (c.placement set); the collision arguments may be null, the hold members are
+// set with a hold mask (track mode).
+inline K1PArgs conv_k1p_args(const ConvCall& c, const ConvBufs& s, int32_t* status) {
+  K1PArgs a;
+  memset(&a, 0, sizeof a);
+  static_cast<K1CArgs&>(a) = conv_k1c_args(c, s, status);
+  if (c.hold) { a.hold = c.hold; a.held = s.held; }
+  a.placement = c.placement;
   return a;
 }
 // K2 of a pass: solves and integrates the instances K1 left undone, and does nothing once the condition said stop.

@@ -229,6 +229,17 @@ class Problem:
             setattr(out, name, t.data_ptr())
         return out, keep
 
+    def _placement(self, placement, q: torch.Tensor, B: int):
+        """Per-instance frame placements as a contiguous [B, F, 7] CUDA tensor of q's dtype (None stays None)."""
+        if placement is None:
+            return None
+        if not self.F:
+            raise ValueError("placement given for a problem without a FrameTask or RelativeFrameTask")
+        t = self.model._dev(placement, dtype=q.dtype)
+        if tuple(t.shape) != (B, self.F, 7):
+            raise ValueError(f"placement must have shape {(B, self.F, 7)} (instances x frame tasks x wxyz_xyz), got {tuple(t.shape)}")
+        return t
+
     def fk_jac(self, q, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2):
         inp, keep, B, q = self._inputs(q, frame_targets, posture_targets, com_targets)
         dev, dt_ = q.device, q.dtype
@@ -278,7 +289,7 @@ class Problem:
 
     def step(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
              damping: float = 1e-12, nsteps: int = 1, integrate: bool = False, dq: Optional[torch.Tensor] = None,
-             status: Optional[torch.Tensor] = None, weights=None, posture_weights=None, bounds=None, collision=None):
+             status: Optional[torch.Tensor] = None, weights=None, posture_weights=None, bounds=None, collision=None, placement=None):
         """solve_ik (x nsteps, optionally integrating q in place).  q: [B,nq] fp32 or fp64 CUDA tensor.
         weights: [B, K] per-instance multipliers in [0, 1] of the frame / CoM task costs, rows in the stacked order of J
         (bik_step_weighted); None: the problem's costs.
@@ -288,7 +299,9 @@ class Problem:
         and VelocityLimit caps per instance on the dofs those limits list (bik_step_bounded; bik.h); None: the problem's.
         collision: (enabled, minimum_distance, detection_distance), each None or enabled [B, npairs] (pair k of instance b is
         used iff != 0) and the distances [B], that replace the CollisionAvoidanceLimit's pairs and distances per instance
-        (bik_step_coll; bik.h); None: the problem's."""
+        (bik_step_coll; bik.h); None: the problem's.
+        placement: [B, F, 7] per-instance poses (wxyz_xyz) of the frame tasks' frames in their tree nodes, tasks in the order of
+        the frame targets, in place of the problem's (bik_step_placed; bik.h); None: the problem's."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
@@ -296,13 +309,18 @@ class Problem:
         pw = self._posture_weights(posture_weights, q, B)
         bd, keep_bd = self._bounds(bounds, q, B)
         co, keep_co = self._collision(collision, q, B)
+        pl = self._placement(placement, q, B)
         if dq is None:
             dq = torch.empty((B, self.nv), device=q.device, dtype=q.dtype)
         if status is None:
             status = torch.empty(B, device=q.device, dtype=torch.int32)
         assert dq.dtype == q.dtype
         args = (float(dt), float(damping), int(nsteps), int(bool(integrate)), dq.data_ptr(), status.data_ptr(), _stream())
-        if co is not None:
+        if pl is not None:
+            fn = self.lib.bik_step_placed64 if _is64(q) else self.lib.bik_step_placed
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd),
+                          None if co is None else C.byref(co), pl.data_ptr(), *args))
+        elif co is not None:
             fn = self.lib.bik_step_coll64 if _is64(q) else self.lib.bik_step_coll
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
         elif bd is not None:
@@ -321,13 +339,14 @@ class Problem:
 
     def converge(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, dt: float = 1e-2,
                  damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
-                 check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None):
+                 check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None, placement=None):
         """solve_ik + integrate until every frame task is within the thresholds or max_iters steps were taken, per instance
         (the inner loop of the reference's examples; bik_converge for a float32 q, bik_converge64 for a float64 q, the
         targets in q's dtype).  q is updated in place.  weights: [B, K] as in `step` (bik_converge_weighted); a frame task
         whose three position (orientation) weights are 0 is left out of the position (orientation) test.
         posture_weights: [B, P, nv] as in `step` (bik_converge_weighted_ex).  bounds: as in `step` (bik_converge_bounded).
-        collision: as in `step` (bik_converge_coll).  Returns (iters [B], status [B])."""
+        collision: as in `step` (bik_converge_coll).  placement: [B, F, 7] as in `step` (bik_converge_placed).
+        Returns (iters [B], status [B])."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         inp, keep, _, _ = self._inputs(None, frame_targets, posture_targets, com_targets, dtype=q.dtype)
         B = q.shape[0]
@@ -335,11 +354,16 @@ class Problem:
         pw = self._posture_weights(posture_weights, q, B)
         bd, keep_bd = self._bounds(bounds, q, B)
         co, keep_co = self._collision(collision, q, B)
+        pl = self._placement(placement, q, B)
         iters = torch.zeros(B, device=q.device, dtype=torch.int32)
         status = torch.zeros(B, device=q.device, dtype=torch.int32)
         args = (float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every), iters.data_ptr(),
                 status.data_ptr(), _stream())
-        if co is not None:
+        if pl is not None:
+            fn = self.lib.bik_converge_placed64 if _is64(q) else self.lib.bik_converge_placed
+            _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd),
+                          None if co is None else C.byref(co), pl.data_ptr(), *args))
+        elif co is not None:
             fn = self.lib.bik_converge_coll64 if _is64(q) else self.lib.bik_converge_coll
             _lib.check(fn(self.handle, B, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd), C.byref(co), *args))
         elif bd is not None:
@@ -359,7 +383,7 @@ class Problem:
     def track(self, q: torch.Tensor, frame_targets=None, posture_targets=None, com_targets=None, lengths=None, dt: float = 1e-2,
               damping: float = 1e-12, max_iters: int = 20, pos_threshold: float = 1e-4, ori_threshold: float = 1e-4,
               check_every: int = 1, weights=None, posture_seq: bool = False, posture_weights=None, bounds=None, collision=None,
-              hold=None):
+              hold=None, placement=None):
         """The converge loop over a sequence of targets, each instance on its own frame cursor (bik_track for a float32 q,
         bik_track64 for a float64 q; the targets and q_traj in q's dtype):
         for every instance b and frame t < lengths[b] (default: all T), what `converge` on frame t's targets gives.
@@ -376,7 +400,8 @@ class Problem:
         hold: [B, T, H] bools, H = F + C + P: the frame-like tasks, then the CoM tasks, then the posture-type tasks, each in
         the order of its targets (bik_track_hold), or None.  Over a run of frames where hold[b, :, k] is set, task k's target
         is its value at the configuration instance b had when the run began (set_target_from_configuration), captured on the
-        device; its target rows on those frames are ignored."""
+        device; its target rows on those frames are ignored.
+        placement: [B, F, 7] as in `converge`, one row per instance for every frame (bik_track_placed), or None."""
         assert q.is_cuda and q.dtype in (torch.float32, torch.float64) and q.is_contiguous()
         m = self.model
         B = q.shape[0]
@@ -404,6 +429,7 @@ class Problem:
             hd = m._dev(hold, torch.uint8)
             if hd.shape != (B, T, H):
                 raise ValueError(f"hold must be [B={B}, T={T}, H={H}] (frame, CoM and posture-type tasks), not {list(hd.shape)}")
+        pl = self._placement(placement, q, B)
         ln = None
         if lengths is not None:
             ln = m._dev(lengths, torch.int32).reshape(-1)
@@ -415,7 +441,11 @@ class Problem:
         passes = torch.zeros(1, device=q.device, dtype=torch.int32)
         args = (_ptr(ln), float(dt), float(damping), int(max_iters), float(pos_threshold), float(ori_threshold), int(check_every),
                 q_traj.data_ptr(), iters.data_ptr(), status.data_ptr(), passes.data_ptr(), _stream())
-        if hd is not None:
+        if pl is not None:
+            fn = self.lib.bik_track_placed64 if _is64(q) else self.lib.bik_track_placed
+            _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd),
+                          None if co is None else C.byref(co), _ptr(hd), pl.data_ptr(), *args))
+        elif hd is not None:
             fn = self.lib.bik_track_hold64 if _is64(q) else self.lib.bik_track_hold
             _lib.check(fn(self.handle, B, T, q.data_ptr(), C.byref(inp), _ptr(w), _ptr(pw), None if bd is None else C.byref(bd),
                           None if co is None else C.byref(co), hd.data_ptr(), *args))

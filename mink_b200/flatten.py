@@ -99,6 +99,7 @@ class FlatModel:
     geom_type: np.ndarray = None
     body_parentid: np.ndarray = None      # MJCF body tree and geom -> body map: what mink_b200.utils walks; None: not recorded
     geom_bodyid: np.ndarray = None
+    site_bodyid: np.ndarray = None        # site -> body map: where a site sits (placement of a site frame); None: not recorded
     geom_contype: np.ndarray = None       # collision filter bits (collision_avoidance_limit.py:269-278); None: not recorded
     geom_conaffinity: np.ndarray = None
     geom_size: np.ndarray = None
@@ -117,6 +118,25 @@ class FlatModel:
         if name not in names:
             raise KeyError(name)
         return table[names.index(name)]
+
+    def frame_body(self, name: str, kind: str) -> int:
+        """MuJoCo body a named body / geom / site frame is fixed to.  ValueError when the model does not record it (a site
+        of a model whose metadata predates site_bodyid)."""
+        i = self.names[kind].index(name)
+        if kind == "body":
+            return i
+        ids = self.site_bodyid if kind == "site" else self.geom_bodyid
+        if ids is None:
+            raise ValueError(f"the model does not record which body each {kind} belongs to")
+        return int(ids[i])
+
+    def placed_frame(self, name: str, kind: str, pos, quat) -> Frame:
+        """The frame `name` of `kind` placed at pose (pos, quat) in its body: what flatten gives the frame of a model whose
+        site_pos / site_quat (geom_pos / geom_quat) hold that pose, composed as flatten's attach composes it.  For a body, a
+        pose in that body (identity: the body itself)."""
+        f = self.body_frames[self.frame_body(name, kind)]
+        p, q = _compose(f.pos, f.quat, np.asarray(pos, dtype=np.float64), np.asarray(quat, dtype=np.float64))
+        return Frame(f.node, p, q)
 
     # ---- blob -------------------------------------------------------------- #
     _SECTIONS = ("node_parent", "node_type", "node_qadr", "node_dadr", "node_pos", "node_quat",
@@ -162,6 +182,7 @@ class FlatModel:
             com_missing=list(self.com_missing or []),
             body_parentid=None if self.body_parentid is None else [int(x) for x in self.body_parentid],
             geom_bodyid=None if self.geom_bodyid is None else [int(x) for x in self.geom_bodyid],
+            site_bodyid=None if self.site_bodyid is None else [int(x) for x in self.site_bodyid],
             geom_contype=None if self.geom_contype is None else [int(x) for x in self.geom_contype],
             geom_conaffinity=None if self.geom_conaffinity is None else [int(x) for x in self.geom_conaffinity]))
 
@@ -196,6 +217,8 @@ class FlatModel:
             if meta.get("body_parentid") is not None:
                 fm.body_parentid = np.array(meta["body_parentid"], dtype=np.int32)
                 fm.geom_bodyid = np.array(meta["geom_bodyid"], dtype=np.int32)
+            if meta.get("site_bodyid") is not None:
+                fm.site_bodyid = np.array(meta["site_bodyid"], dtype=np.int32)
             if meta.get("geom_contype") is not None:
                 fm.geom_contype = np.array(meta["geom_contype"], dtype=np.int32)
                 fm.geom_conaffinity = np.array(meta["geom_conaffinity"], dtype=np.int32)
@@ -327,6 +350,7 @@ def flatten(model) -> FlatModel:
     fm.geom_type = np.asarray(model.geom_type).astype(np.int32)
     fm.body_parentid = np.asarray(model.body_parentid).astype(np.int32)
     fm.geom_bodyid = np.asarray(model.geom_bodyid).astype(np.int32)
+    fm.site_bodyid = np.asarray(model.site_bodyid).astype(np.int32)
     if getattr(model, "geom_contype", None) is not None:
         fm.geom_contype = np.asarray(model.geom_contype).astype(np.int32)
         fm.geom_conaffinity = np.asarray(model.geom_conaffinity).astype(np.int32)

@@ -225,6 +225,57 @@ def _collision(limits: Optional[Sequence[Limit]], collision, q, T: Optional[int]
             None if ddet is None else per_instance(ddet, (), q.dtype, "collision_detection_distance"))
 
 
+def _frame_row(frame, dtype):
+    """A frame's pose in its node as the problem image holds it (bik_build.h put_frame): the position, and the quaternion
+    divided by its norm in double, then both in `dtype`."""
+    import math
+
+    q = [float(x) for x in frame.quat]
+    n = math.sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3])
+    n = n if n > 0 else 1.0
+    return np.array([x / n for x in q] + [float(x) for x in frame.pos], dtype=np.float64).astype(dtype)
+
+
+def _placement(tasks: Sequence[Task], placement, q, flat):
+    """The [B, F, 7] placement buffer of a `placement={task: pose}` mapping, F the FrameTask / RelativeFrameTask of the task
+    list in list order: each task's frame in its tree node, the problem's own for tasks the mapping leaves out; None for no
+    mapping.  A pose is an SE3, a [7] or a [B, 7] array or tensor (wxyz_xyz) of the frame in its body, as model.site_pos /
+    site_quat (geom_pos / geom_quat) hold it; it is composed with the body's pose in its node in fp64 as flatten composes a
+    site (or geom), then stored in q's dtype as the problem image stores a frame."""
+    if not placement:
+        return None
+    import torch
+
+    for task in placement:
+        if not isinstance(task, FrameTask) or not any(task is t for t in tasks):
+            raise InvalidTarget(f"placement applies to the FrameTask and RelativeFrameTask of the task list, not {type(task).__name__}")
+    B = q.shape[0]
+    dt = np.float64 if q.dtype == torch.float64 else np.float32
+    rows = []
+    for task in tasks:
+        if not isinstance(task, FrameTask):
+            continue
+        pose = placement.get(task)
+        if pose is None:
+            rows.append(np.broadcast_to(_frame_row(task._spec(flat).frame, dt), (B, 7)))
+            continue
+        if hasattr(pose, "wxyz_xyz"):
+            pose = pose.wxyz_xyz
+        p = pose.detach().cpu().numpy() if isinstance(pose, torch.Tensor) else np.asarray(pose)
+        p = p.astype(np.float64)
+        if p.shape not in ((7,), (B, 7)):
+            raise InvalidTarget(f"Expected a placement of shape [7] or [{B}, 7] for {type(task).__name__}, got {list(p.shape)}")
+        try:
+            flat.frame_body(task.frame_name, task.frame_type)
+        except (KeyError, ValueError) as e:
+            raise InvalidTarget(f"cannot place the frame of {type(task).__name__} {task.frame_name!r}: {e}") from None
+        p = p.reshape(-1, 7)
+        uniq, inv = np.unique(p, axis=0, return_inverse=True)   # the composition is per distinct pose
+        placed = np.stack([_frame_row(flat.placed_frame(task.frame_name, task.frame_type, u[4:], u[:4]), dt) for u in uniq])
+        rows.append(np.broadcast_to(placed[inv.reshape(-1)], (B, 7)))
+    return torch.as_tensor(np.ascontiguousarray(np.stack(rows, axis=1)), device=q.device)
+
+
 def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, damping: float = 1e-12,
              limits: Optional[Sequence[Limit]] = None) -> Problem:
     """QP of the IK problem (reference solve_ik.py:43-65): P = damping I + sum H_t, q = sum c_t,
@@ -251,7 +302,7 @@ def build_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, dam
 
 def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
              safety_break: bool = False, limits: Optional[Sequence[Limit]] = None, weights=None, posture_weights=None, bounds=None,
-             collision=None, **kwargs):
+             collision=None, placement=None, **kwargs):
     """Velocity v = dq / dt tangent to the configuration (reference solve_ik.py:68-105).
 
     `weights` maps a FrameTask / RelativeFrameTask to a [6] or [B, 6] array and a ComTask to a [3] or [B, 3] array of
@@ -277,6 +328,13 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     replace the limit's attributes of those names per instance; a non-finite distance keeps the limit's own and flags the
     instance.  compute_qp_inequalities still shows the limit's own pairs and distances.
 
+    `placement` maps a FrameTask / RelativeFrameTask of `tasks` to the pose of its frame in its body, an SE3 or a [7] or
+    [B, 7] array (wxyz_xyz): what model.site_pos / site_quat (geom_pos / geom_quat) hold for a site (geom) frame, a pose in
+    the body for a body frame (identity: the body itself).  Instance b solves as if the model had been built with its
+    frame there: one marker placement per performer, one tool length per instance, one contact point per grasp.  A
+    RelativeFrameTask's root keeps its place, and tasks left out keep the model's.  Task.compute_error / compute_jacobian
+    still use the model's placement.
+
     Returns a numpy (nv,) vector for a single configuration, a torch CUDA [B, nv] tensor for a batch.
     Raises NotWithinConfigurationLimits when `safety_break` and some instance is out of limits;
     raises AssertionError (like the reference's `assert dq is not None`) when the QP of any instance
@@ -289,8 +347,9 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
     bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
     co = _collision(limits_arg, collision, q)
+    pl = _placement(tasks, placement, q, configuration.flat)
     dq, status = prob.step(q, dt=dt, damping=damping, nsteps=1, integrate=False, weights=w, posture_weights=pw, bounds=bd, collision=co,
-                           **kw)
+                           placement=pl, **kw)
     st = status.cpu().numpy()
     if (st & 1).any():
         if safety_break:
@@ -306,7 +365,8 @@ def solve_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, sol
 
 def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, solver: str = "b200", damping: float = 1e-12,
                 limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
-                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None):
+                ori_threshold: float = 1e-4, check_every: int = 1, weights=None, posture_weights=None, bounds=None, collision=None,
+                placement=None):
     """The inner loop the reference's examples wrap around solve_ik (examples/arm_iiwa.py:63-70,
     examples/quadruped_spot.py:89-104), run on the device per instance:
 
@@ -320,7 +380,8 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     batch run in fp64 end to end (bik_converge64), a float32 batch on the fp32 fast path.
 
     `weights` as in solve_ik.  A frame task whose three position (orientation) weights are 0 in an instance is left out of
-    that instance's position (orientation) test.  `posture_weights`, `bounds` and `collision` as in solve_ik."""
+    that instance's position (orientation) test.  `posture_weights`, `bounds`, `collision` and `placement` as in solve_ik;
+    the thresholds are tested on the placed frames' errors."""
     limits_arg = limits   # the caller's list: `bounds` and `collision` keys name its limits
     prob, kw, limits = _lower(configuration, tasks, limits)
     q = configuration.q_device
@@ -328,9 +389,10 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
     pw = _posture_weights(tasks, posture_weights, q, configuration.flat.nv)
     bd = _limit_bounds(limits_arg, bounds, q, configuration.flat)
     co = _collision(limits_arg, collision, q)
+    pl = _placement(tasks, placement, q, configuration.flat)
     iters, status = prob.converge(q, dt=dt, damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
                                   ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_weights=pw, bounds=bd,
-                                  collision=co, **kw)
+                                  collision=co, placement=pl, **kw)
     configuration._sync_from_device()
     st = status.cpu().numpy()
     assert not (st & _QP_BITS).any(), f"QP not solved for {int(((st & _QP_BITS) != 0).sum())} instance(s) (status bits {np.unique(st & _QP_BITS)})"
@@ -343,7 +405,7 @@ def converge_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, 
 def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, targets, solver: str = "b200",
              damping: float = 1e-12, limits: Optional[Sequence[Limit]] = None, max_iters: int = 20, pos_threshold: float = 1e-4,
              ori_threshold: float = 1e-4, lengths=None, check_every: int = 1, weights=None, posture_weights=None, bounds=None,
-             collision=None, hold=None):
+             collision=None, hold=None, placement=None):
     """The examples' outer loop (examples/arm_aloha.py:140-169) over a sequence of targets, run on the device:
 
         for t in range(T):
@@ -382,6 +444,9 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     where it touched down for as long as the contact lasts.  The value is captured on the device; it replaces the task's
     sequence or target on the held frames.  A task held on every frame of every instance needs neither a sequence nor a
     target.  A DampingTask cannot be held.
+
+    `placement` as in solve_ik, one pose per instance that holds on every frame (a performer's markers, a tool).  A held
+    FrameTask captures the world pose of its placed frame, a held RelativeFrameTask that frame's pose in its root.
 
     Returns (q_traj, iters, converged) per frame: numpy float64 [T, nq] / [T] / [T] for a single configuration, torch
     CUDA [B, T, nq] (q's dtype) / [B, T] / [B, T] for a batch (rows past an instance's length: NaN, -1, False)."""
@@ -467,6 +532,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     pw = _posture_weights(tasks, posture_weights, q, flat.nv, T)
     bd = _limit_bounds(limits_arg, bounds, q, flat)
     co = _collision(limits_arg, collision, q, T)
+    pl = _placement(tasks, placement, q, flat)
     ln = None
     if lengths is not None:
         ln = lengths.to(device=dev, dtype=torch.int32) if isinstance(lengths, torch.Tensor) else torch.as_tensor(np.asarray(lengths, dtype=np.int32), device=dev)
@@ -483,7 +549,7 @@ def track_ik(configuration: Configuration, tasks: Sequence[Task], dt: float, tar
     q_traj, iters, status, _ = prob.track(q, stacked(FrameTask, 7), posture, stacked(ComTask, 3), lengths=ln, dt=dt,
                                           damping=damping, max_iters=max_iters, pos_threshold=pos_threshold,
                                           ori_threshold=ori_threshold, check_every=check_every, weights=w, posture_seq=posture_seq,
-                                          posture_weights=pw, bounds=bd, collision=co, hold=hd)
+                                          posture_weights=pw, bounds=bd, collision=co, hold=hd, placement=pl)
     configuration._sync_from_device()
     ran = iters >= 0
     bad = ((status & _QP_BITS) != 0) & ran
